@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """
-bench.py -- rays/sec of the pixelNeRF render hot path on B200 (BASELINE.json metric).
+bench.py -- rays/sec of the pixelNeRF render hot path on H100 (BASELINE.json metric).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c3|c4] [--scaling weak|strong]
-                  [--impl ours|reference|reference-gpu|torch-eager]
+                  [--impl ours|reference|reference-gpu|torch-eager] [--dump-outputs DIR]
   torchrun --nproc-per-node N ... bench.py --gpus N ...   (one rank per GPU, NCCL)
 
 A "step" renders one batch of synthetic rays (coarse + fine pass) of a BASELINE.json workload:
@@ -15,16 +15,21 @@ so the random network renders a non-blank, semi-transparent volume), and a real 
 (`NeRFRenderer.bind_parallel(net)(rays)`) from pinned HOST rays to HOST pixels.
 
 Ranks shard rays (render/sharding.py, torch.chunk order): `--scaling weak` (default) gives every GPU one frame,
-`--scaling strong` splits ONE frame over the N GPUs (BASELINE configs C3 / C4: "8xB200 ray-sharded").  The scene is
+`--scaling strong` splits ONE frame over the N GPUs (BASELINE configs C3 / C4: "N-GPU ray-sharded").  The scene is
 broadcast from rank 0 once (NCCL) and rendered pixels are gathered to rank 0 every step inside the timed region.
 
 The line also carries a `parity` block: the benchmarked model + frame, 256 rays with injected noise, CUDA vs the CPU
 oracle (outside the timed region).
 
-`--impl reference` times the UNMODIFIED reference (baseline/_ref, installed by scripts/install_ref.py; falls back to the
+`--impl reference` times the UNMODIFIED reference (oracle/_ref, installed by oracle/install_ref.py; falls back to the
 oracle port when absent) on the HOST CPU cores through its own public API, on a bounded sample of the same workload;
-`--impl reference-gpu` runs the same unmodified reference eagerly on the B200(s) (fp32, TF32 off; DataParallel at N>1) --
+`--impl reference-gpu` runs the same unmodified reference eagerly on the GPU(s) (fp32, TF32 off; DataParallel at N>1) --
 the denominator of north_star's ">= 10x the reference's own 1xGPU PyTorch rays/sec".
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (rank 0, gathered): DIR/rgb.npy
+(1, rays, 3) and DIR/depth.npy (1, rays), float32; above 64 MB in all, a fixed seeded sample of rays plus their ray
+numbers (DIR/ray_index.npy).  Rays, weights and sampling noise are seeded, so two builds run with the same arguments
+can be compared output for output.
 """
 import argparse
 import importlib.util
@@ -65,49 +70,12 @@ WORKLOADS = {
 }
 
 
-def profile_file(workload):
-    for name in (f"r2_k_field_tc_{workload}.txt", "r2_k_field_tc.txt", "r1_final_k_field_tc.txt"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p) and (workload == "c2" or name.startswith(f"r2_k_field_tc_{workload}")):
-            return p
-    return None
-
-
-def profiled_traffic(workload):
-    """dram bytes per launch of the dominant kernel from the committed ncu capture of this command; None if absent."""
-    p = profile_file(workload)
-    if p is None:
-        return None, None
-    n, tot = 0, 0.0
-    for line in open(p):
-        if "dram__bytes_read.sum [" in line or "dram__bytes_write.sum [" in line:
-            unit = line.split("[")[1].split("]")[0]
-            val = float(line.split("=")[1])
-            tot += val * {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}.get(unit, 1)
-            n += 1
-    return (tot / (n / 2) if n else None), os.path.relpath(p, ROOT)
-
-
-def profiled_tensor_active(workload):
-    p = profile_file(workload)
-    if p is None:
-        return None
-    vals = [float(l.split("=")[1]) for l in open(p)
-            if "sm__pipe_tensor_cycles_active_realtime.avg.pct_of_peak_sustained_elapsed" in l]
-    return sum(vals) / len(vals) if vals else None
-
-
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0)), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
-    return 1400.0, "fallback (B200_PROFILING.md sustained)"
+    return 989.0, "H100 SXM data sheet, dense FP16 (not a measured rate)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index=0):
         super().__init__(daemon=True)
@@ -231,6 +199,25 @@ def parity_block(net, renderer, cfg, rays_dev, n=256):
             "oracle_seconds": t_oracle}
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, rgb, depth):
+    """rgb (1, R, 3) and depth (1, R) as float32 .npy.  Above DUMP_LIMIT_BYTES in all, a fixed seeded sample of rays
+    (sorted) is written instead, with the sampled ray numbers as ray_index.npy (float64, exact)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    R = rgb.shape[1]
+    per_ray = 4 * 4                                   # rgb + depth, float32
+    if R * per_ray > DUMP_LIMIT_BYTES:
+        keep = (DUMP_LIMIT_BYTES - 4096) // (per_ray + 8)   # + the float64 ray number; 4 KB for the .npy headers
+        idx = torch.randperm(R, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        rgb, depth = rgb[:, idx.to(rgb.device)], depth[:, idx.to(depth.device)]
+        np.save(os.path.join(out_dir, "ray_index.npy"), idx.double().numpy())
+    np.save(os.path.join(out_dir, "rgb.npy"), rgb.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "depth.npy"), depth.detach().float().cpu().numpy())
+
+
 def run_ours(args):
     if SRC not in sys.path:
         sys.path.insert(0, SRC)
@@ -264,7 +251,7 @@ def run_ours(args):
     my_rays_host = sharding.local_shard(all_rays, rank, world, dim=1)[0].contiguous().pin_memory()
     n_mine = my_rays_host.shape[0]
     rays_dev = my_rays_host.to(device)[None]                      # (1, n_mine, 8) resident
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=device)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=device)  # > 50 MB L2
 
     def gather(rgb, depth):
         if dist is None:
@@ -272,11 +259,13 @@ def run_ours(args):
         return (sharding.gather_rays(rgb, total, dist, rank, world, dst=0, dim=1),
                 sharding.gather_rays(depth, total, dist, rank, world, dst=0, dim=1))
 
+    last = {}
+
     def step_resident():
         flush.zero_()
         with torch.no_grad():
             rgb, depth = render_par(rays_dev)
-        return gather(rgb, depth)
+        last["rgb"], last["depth"] = gather(rgb, depth)
 
     host_rgb = torch.empty(1, total if rank == 0 else 1, 3).pin_memory()
     host_dep = torch.empty(1, total if rank == 0 else 1).pin_memory()
@@ -319,11 +308,9 @@ def run_ours(args):
     pn.profile_begin()
     ms_total = timed(step_resident, args.steps)
     kern_ms, kern_launches = pn.profile_end()
-    if os.environ.get("PNR_TC_COUNTERS"):
-        names = ["mma_total", "mma_wait_a_first_chunk", "mma_wait_b", "mma_wait_bpeer", "unused4", "unused5",
-                 "mma_wait_a_later_chunks", "stream_wait_empty"]
-        print("tc_counters", dict(zip(names, pn.tc_counters())), file=sys.stderr)
     launches = pn.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["rgb"], last["depth"])
     for _ in range(2):
         step_e2e()
     ms_e2e = timed(step_e2e, args.steps)
@@ -355,7 +342,6 @@ def run_ours(args):
         cpu_base = cpu_baseline_subprocess(args.workload, args.cpu_rays or wl["cpu_rays"])
 
     if rank == 0:
-        traffic, traffic_src = profiled_traffic(args.workload)
         line = {
             "metric": wl["metric"], "value": value, "unit": "rays/s", "n_gpus": world, "steps": args.steps,
             "warmup": warm, "ms_per_step": ms_total / args.steps, "higher_is_better": True,
@@ -371,11 +357,8 @@ def run_ours(args):
                     "d2h_bytes_per_step": total * 4 * 4},
             "gpu_launches": int(launches),
             "roofline": {"bound": "tensor", "achieved": kern_tflops, "peak": peak, "unit": "TFLOP/s",
-                         "frac": (kern_tflops / peak) if kern_tflops else None, "traffic": traffic,
+                         "frac": (kern_tflops / peak) if kern_tflops else None,
                          "peak_source": peak_src, "kernel_launches": int(kern_launches),
-                         "ncu_tensor_pipe_active_pct": profiled_tensor_active(args.workload),
-                         "traffic_note": f"dram bytes per launch from {traffic_src} (same command under ncu); see "
-                                         "DESIGN.md section 7 for what they consist of",
                          "kernel_ms_per_step": kern_ms / args.steps,
                          "executed_fp16_mma_tflops": exec_tflops if tensor_engine else None,
                          "executed_frac_of_peak": (exec_tflops / peak) if (tensor_engine and exec_tflops) else None,
@@ -393,10 +376,10 @@ def run_ours(args):
 
 
 # ------------------------------------------------------------------------------------------
-# reference arms: the UNMODIFIED reference through its own public API (baseline/_ref)
+# reference arms: the UNMODIFIED reference through its own public API (oracle/_ref)
 # ------------------------------------------------------------------------------------------
 def reference_root():
-    for root in (os.environ.get("PIXELNERF_REF"), os.path.join(ROOT, "baseline", "_ref")):
+    for root in (os.environ.get("PIXELNERF_REF"), os.path.join(ROOT, "oracle", "_ref")):
         if root and os.path.isdir(os.path.join(root, "src", "render")):
             return root
     return None
@@ -404,7 +387,7 @@ def reference_root():
 
 def build_reference_scene(workload, device):
     """The reference's PixelNeRFNet + NeRFRenderer + bind_parallel, weights and scene of the workload; returns
-    (net, renderer) or None when baseline/_ref is absent."""
+    (net, renderer) or None when oracle/_ref is absent."""
     root = reference_root()
     if root is None:
         return None
@@ -457,7 +440,7 @@ def cpu_arm(workload):
         def render(rays):
             with torch.no_grad():
                 return render_par(rays)
-        kind, what = "reference", "unmodified reference (baseline/_ref) NeRFRenderer.bind_parallel(net)(rays), torch CPU fp32"
+        kind, what = "reference", "unmodified reference (oracle/_ref) NeRFRenderer.bind_parallel(net)(rays), torch CPU fp32"
     else:
         oracle = _load("pnr_oracle", os.path.join(ROOT, "oracle", "pnr_oracle.py"))
         src, _, focal, c = synth.make_cameras(cfg)
@@ -470,7 +453,7 @@ def cpu_arm(workload):
             with torch.no_grad():
                 return oracle.render(rays, noise, state, latent, wc, wf, cfg["NS"], cfg["n_coarse"], cfg["n_fine"],
                                      cfg["n_fine_depth"], white_bkgd=cfg["white_bkgd"], eval_batch_size=50000)
-        kind, what = "port", "oracle/pnr_oracle.py (baseline/_ref absent), torch CPU fp32"
+        kind, what = "port", "oracle/pnr_oracle.py (oracle/_ref absent), torch CPU fp32"
     ncpu = os.cpu_count() or 1
     cands = sorted({t for t in (8, 16, 32, 64, 128, ncpu) if t <= ncpu})
     probe_rays = synth.make_rays(cfg, 64)[None]
@@ -532,7 +515,7 @@ def run_reference(args):
 
 
 def run_reference_gpu(args):
-    """Context arm: the unmodified reference, eager PyTorch fp32 (TF32 off), on the B200(s): `net.cuda()`,
+    """Context arm: the unmodified reference, eager PyTorch fp32 (TF32 off), on the GPU(s): `net.cuda()`,
     `bind_parallel(net, gpus)` = nn.DataParallel(dim=1) when N > 1 (reference src/render/nerf.py:354-371), rays split in
     `ray_batch_size` = 50 000 pieces like eval/gen_video.py:213-216.  Single process (rank 0 only under torchrun)."""
     rank = int(os.environ.get("RANK", "0"))
@@ -541,7 +524,7 @@ def run_reference_gpu(args):
     wl = WORKLOADS[args.workload]
     cfg = synth.CONFIGS[args.workload]
     if reference_root() is None:
-        print(json.dumps({"impl": "reference-gpu", "unavailable": "baseline/_ref not installed (scripts/install_ref.py)"}))
+        print(json.dumps({"impl": "reference-gpu", "unavailable": "oracle/_ref not installed (oracle/install_ref.py)"}))
         return
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
@@ -578,7 +561,7 @@ def run_reference_gpu(args):
                       "dtype": "f32 (TF32 off)", "data": "synthetic",
                       "config": {"workload": wl["text"], "rays_per_step": total, "ray_batch_size": 50000,
                                  "parallelism": "single GPU" if args.gpus == 1 else f"nn.DataParallel(dim=1) x{args.gpus}",
-                                 "note": "unmodified reference (baseline/_ref), PyTorch eager"}}))
+                                 "note": "unmodified reference (oracle/_ref), PyTorch eager"}}))
 
 
 def run_torch_eager(args):
@@ -635,6 +618,8 @@ if __name__ == "__main__":
     ap.add_argument("--cpu-rays", type=int, default=0, help="rays per CPU-reference pass (default per workload)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's rgb / depth as DIR/<name>.npy (float32)")
     a = ap.parse_args()
     if a.impl == "reference":
         run_reference(a)

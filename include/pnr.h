@@ -1,5 +1,5 @@
 /*
- * pnr.h -- C ABI of libpnr_sm100.so, the B200-native replacement for pixelNeRF's
+ * pnr.h -- C ABI of libpnr_sm90.so, the H100-native (sm_90a) replacement for pixelNeRF's
  * volume-rendering hot path.
  *
  * The reference (sxyu/pixel-nerf) is 100 % Python/PyTorch and has no FFI of its own, so
@@ -41,7 +41,7 @@ enum {
 enum {
   PNR_ENGINE_AUTO = 0,   /* tensor engine when the shape allows it, else SIMT            */
   PNR_ENGINE_SIMT = 1,   /* fp32 FFMA kernels, any shape (bring-up / small-d engine)      */
-  PNR_ENGINE_TC = 2      /* tcgen05 split-fp16 (3 products, fp32 accumulate) fused kernel */
+  PNR_ENGINE_TC = 2      /* wgmma split-fp16 (3 products, fp32 accumulate) fused kernel */
 };
 
 /* State left behind by PixelNeRFNet.encode (src/model/models.py:89-144) and
@@ -82,7 +82,7 @@ typedef struct PnrMlp {
   const float* fc0_b[PNR_MAX_BLOCKS];
   const float* fc1_w[PNR_MAX_BLOCKS];
   const float* fc1_b[PNR_MAX_BLOCKS];
-  /* tensor engine only: fp16 hi/lo split, UMMA-tiled weights from pnr_pack_mlp (else NULL) */
+  /* tensor engine only: fp16 hi/lo split, wgmma-tiled weights from pnr_pack_mlp (else NULL) */
   const void* packed;
   size_t packed_bytes;
 } PnrMlp;
@@ -168,7 +168,7 @@ int pnr_field_eval(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, c
  *   grad          : a PnrMlp whose weight pointers are WRITABLE gradient buffers of the same shapes; accumulated (+=)
  *   d_latent_nhwc : [V][Hl][Wl][C] channels-last gradient of the latent; accumulated (+=); may be NULL
  *   d_xyz         : [SB][P][3] gradient of the sample positions (overwritten); may be NULL
- * Recompute-in-backward (arithmetic = oracle/pnr_backward.py); the GEMMs run on the tensor cores (split-bf16 tcgen05,
+ * Recompute-in-backward (arithmetic = oracle/pnr_backward.py); the GEMMs run on the tensor cores (split-bf16 wgmma,
  * PNR_BWD_GEMM=simt selects the fp32 FFMA SGEMM).  This is what PixelNeRFNet.forward's autograd node calls on CUDA. */
 size_t pnr_field_backward_workspace_bytes(const PnrScene* scene, const PnrMlp* mlp, int64_t P);
 int pnr_field_backward(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
@@ -183,7 +183,7 @@ int pnr_field_backward(const PnrScene* scene, const PnrMlp* mlp, const float* xy
  *   d_latent_nhwc: [V][Hl][Wl][C], accumulated (+=); may be NULL
  * The coarse weights are detached for importance sampling but the coarse depth is not (nerf.py:286-291), so the fine
  * loss also reaches the coarse MLP.  Gradients w.r.t. the depth / weights outputs are not supported.
- * Arithmetic = oracle/pnr_backward.py::train_loss_backward; validated on B200 against the reference's own gradients.
+ * Arithmetic = oracle/pnr_backward.py::train_loss_backward; validated on H100 against the reference's own gradients.
  * This is the backward of the default CUDA training path (NeRFRenderer.forward in grad mode). */
 size_t pnr_render_backward_workspace_bytes(const PnrScene* scene, const PnrMlp* mlp_coarse,
                                            const PnrMlp* mlp_fine, const PnrRenderCfg* cfg, int64_t B);
@@ -204,7 +204,8 @@ int pnr_render(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* ml
                void* stream);
 
 /* Tensor-engine preparation (once per weight version / per encode()):
- *  - pnr_pack_mlp: fp32 nn.Linear weights -> fp16 hi/lo split, K-major 128B-swizzled UMMA tiles.
+ *  - pnr_pack_mlp: fp32 nn.Linear weights -> fp16 hi/lo split, K-major 128B-swizzled wgmma tiles
+ *    (128 output rows x 64 k, in the order the fused kernel consumes them).
  *  - pnr_project_latent: proj[i][v][y][x][:] = lin_z[i](latent[v,:,y,x]) (+ bias), so that the
  *    per-sample lin_z GEMMs (resnetfc.py:175) become a bilinear gather of the projected map
  *    (bilinear interpolation commutes with a linear layer). */
@@ -248,7 +249,7 @@ int pnr_mgpu_render(PnrMgpu* h, const PnrShard* shards, const PnrRenderCfg* cfg,
 
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.
- * engine = PNR_ENGINE_SIMT: fp32 FFMA SGEMM; PNR_ENGINE_TC (or AUTO): split-bf16 tcgen05 GEMM (3 products, fp32
+ * engine = PNR_ENGINE_SIMT: fp32 FFMA SGEMM; PNR_ENGINE_TC (or AUTO): split-bf16 wgmma GEMM (3 products, fp32
  * accumulate, split-K with atomics when the output has few tiles) -- the backward's engine; PNR_GEMM_F16X3: the same
  * kernel with fp16 hi/lo operands (22 mantissa bits inside fp16's range) -- pnr_project_latent's engine.
  * K % 16 == 0, rows 16-byte aligned. */
@@ -259,7 +260,7 @@ int pnr_gemm_nt(const float* A, int32_t lda, const float* W, const float* bias, 
 /* How many kernels this library has launched in this process (bench.py "gpu_launches"). */
 int64_t pnr_launch_count(void);
 
-/* Device-time profile of the DOMINANT kernel (the MLP contraction: the fused tcgen05 kernel of
+/* Device-time profile of the DOMINANT kernel (the MLP contraction: the fused wgmma kernel of
  * the tensor engine, or the SGEMM of the SIMT engine).  Between begin and end every launch of
  * that kernel is bracketed by cudaEvents on its own stream; end synchronises those events and
  * returns the summed device milliseconds and the number of launches.  Off by default. */

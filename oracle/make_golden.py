@@ -13,6 +13,7 @@ these files are what pins the oracle.
 """
 import argparse
 import importlib.util
+import json
 import os
 import sys
 
@@ -239,6 +240,60 @@ def frames_fixture():
     print("frames_u8: written")
 
 
+def _flatten_conf(c, prefix=""):
+    out = {}
+    for k in c.keys():
+        v = c[k]
+        if hasattr(v, "keys"):
+            out.update(_flatten_conf(v, prefix + k + "."))
+        else:
+            out[prefix + k] = v
+    return out
+
+
+def conf_fixture():
+    """The reference's conf/exp/*.conf and expconf.conf as flattened trees, read with this package's HOCON reader (the
+    reference's files are the schema the shipped confs must equal)."""
+    hocon = _load("pnr_hocon", os.path.join(ROOT, "pixel-nerf_b200", "src", "util", "hocon.py"))
+    ref = ref_harness.REF_ROOT
+    rec = {"exp/" + name: _flatten_conf(hocon.parse_file(os.path.join(ref, "conf", "exp", name)))
+           for name in sorted(os.listdir(os.path.join(ref, "conf", "exp")))}
+    rec["expconf.conf"] = _flatten_conf(hocon.parse_file(os.path.join(ref, "expconf.conf")))
+    path = os.path.join(GOLD, "ref_confs.json")
+    with open(path, "w") as f:
+        json.dump(rec, f, indent=1, sort_keys=True)
+    print(f"ref_confs: wrote {path} ({len(rec)} files)")
+
+
+def encode_fixture():
+    """The reference's SpatialEncoder.forward / PixelNeRFNet.encode state (src/model/encoder.py:111-164,
+    src/model/models.py:89-144) for oracle.seeded_state weights on oracle.encode_scene inputs: the camera state exactly,
+    the latent and index() values at oracle.encode_sample_index positions, and their max |value| (tolerance scale)."""
+    model, _, _ = ref_harness.import_reference()
+    rec = {}
+    for name, (use_first_pool, (SB, NS, H, W)) in oracle.ENCODE_CASES.items():
+        net = model.make_model(ref_harness.model_conf(64, use_first_pool)).eval()
+        net.load_state_dict(oracle.seeded_state(net.state_dict(), 3), strict=True)
+        images, poses, focal, c, uv = oracle.encode_scene(7, SB, NS, H, W)
+        with torch.no_grad():
+            net.encode(images, poses, focal, c=c)
+            idx = net.encoder.index(uv, None, net.image_shape)
+        lat = net.encoder.latent
+        rec[name + "/latent_shape"] = np.array(lat.shape)
+        rec[name + "/latent"] = lat.reshape(-1)[oracle.encode_sample_index(lat.numel(), 1)].numpy()
+        rec[name + "/latent_absmax"] = np.array(lat.abs().max().item())
+        rec[name + "/index_shape"] = np.array(idx.shape)
+        rec[name + "/index"] = idx.reshape(-1)[oracle.encode_sample_index(idx.numel(), 2)].numpy()
+        rec[name + "/index_absmax"] = np.array(idx.abs().max().item())
+        for k in ("latent_scaling", "poses", "focal", "c", "image_shape"):
+            v = net.encoder.latent_scaling if k == "latent_scaling" else getattr(net, k)
+            rec[name + "/" + k] = v.numpy()
+        rec[name + "/num_views_per_obj"] = np.array(net.num_views_per_obj)
+    path = os.path.join(GOLD, "encode_state.npz")
+    np.savez_compressed(path, **rec)
+    print(f"encode_state: wrote {path} ({os.path.getsize(path) / 1e3:.0f} KB)")
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--check", action="store_true")
@@ -254,6 +309,10 @@ if __name__ == "__main__":
         util_fixture(a.check)
     if not a.only or a.only == "frames_u8":
         frames_fixture()
+    if not a.only or a.only == "confs":
+        conf_fixture()
+    if not a.only or a.only == "encode_state":
+        encode_fixture()
     if not a.only or a.only == "grad":
         grad_fixture("tiny", a.check)
         grad_fixture("sb2_d", a.check)

@@ -310,3 +310,51 @@ def frames_u8(rgb):
     Defined for values in [0, 256/255) only (the cast is implementation-defined outside)."""
     import numpy as np
     return (rgb.detach().cpu().numpy().astype(np.float32) * 255).astype(np.uint8)
+
+
+# ------------------------------------------------------------------------------------------
+# encode() state fixture (tests/golden/encode_state.npz): a seeded model state and scene that the reference and this
+# package can both load, so the reference's encode() outputs can be stored without storing the trunk's weights
+# ------------------------------------------------------------------------------------------
+ENCODE_CASES = {"pool": (True, (2, 2, 48, 64)), "nopool": (False, (1, 3, 40, 40))}
+ENCODE_SAMPLES = 4096
+
+
+def seeded_state(template, seed):
+    """A state_dict with the keys and shapes of `template`, filled from a generator in key order: weights ~ N(0, 1/fan_in),
+    BatchNorm affine near (1, 0), running stats away from their (0, 1) initial values so eval-mode BN does real work."""
+    g = torch.Generator().manual_seed(seed)
+    out = {}
+    for k in sorted(template):
+        t = template[k]
+        if not t.is_floating_point():
+            out[k] = t.clone()
+        elif k.endswith("running_var"):
+            out[k] = torch.rand(t.shape, generator=g) + 0.5
+        elif k.endswith("running_mean") or k.endswith("bias"):
+            out[k] = torch.randn(t.shape, generator=g) * 0.1
+        elif t.dim() == 1:                                   # BatchNorm weight
+            out[k] = 1.0 + torch.randn(t.shape, generator=g) * 0.1
+        else:
+            fan_in = t[0].numel()
+            out[k] = torch.randn(t.shape, generator=g) / math.sqrt(fan_in)
+    return out
+
+
+def encode_scene(seed, SB, NS, H, W):
+    """images (SB,NS,3,H,W) in [-1,1], c2w poses, focal (SB,2), c (SB,2) and index() query points uv (SB*NS,33,2)."""
+    g = torch.Generator().manual_seed(seed)
+    images = torch.rand(SB, NS, 3, H, W, generator=g) * 2 - 1
+    poses = torch.eye(4).repeat(SB, NS, 1, 1)
+    poses[..., :3, :3] = torch.linalg.qr(torch.randn(SB, NS, 3, 3, generator=g))[0]
+    poses[..., :3, 3] = torch.randn(SB, NS, 3, generator=g)
+    focal = torch.rand(SB, 2, generator=g) * 50 + 40
+    c = torch.rand(SB, 2, generator=g) * 4 + torch.tensor([W / 2.0, H / 2.0])
+    uv = torch.rand(SB * NS, 33, 2, generator=g) * torch.tensor([W * 1.2, H * 1.2]) - 3.0
+    return images, poses, focal, c, uv
+
+
+def encode_sample_index(numel, seed):
+    """Fixed positions at which the fixture stores the (large) latent / index() outputs."""
+    g = torch.Generator().manual_seed(seed)
+    return torch.randperm(numel, generator=g)[:ENCODE_SAMPLES]

@@ -19,9 +19,9 @@ _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _find_ref():
-    """$PIXELNERF_REF, else /root/reference (this container), else baseline/_ref (the copy scripts/install_ref.py ships
+    """$PIXELNERF_REF, else /root/reference (this container), else oracle/_ref (the copy oracle/install_ref.py ships
     to the GPU box for the timing arms of bench.py)."""
-    for root in (os.environ.get("PIXELNERF_REF"), "/root/reference", os.path.join(_REPO, "baseline", "_ref")):
+    for root in (os.environ.get("PIXELNERF_REF"), "/root/reference", os.path.join(_REPO, "oracle", "_ref")):
         if root and os.path.isdir(os.path.join(root, "src")):
             return root
     return "/root/reference"

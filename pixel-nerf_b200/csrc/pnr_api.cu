@@ -1,4 +1,4 @@
-// C-ABI entry points of libpnr_sm100.so (see include/pnr.h).  Thin: argument checks, engine
+// C-ABI entry points of libpnr_sm90.so (see include/pnr.h).  Thin: argument checks, engine
 // selection, workspace carving, and the coarse -> fine orchestration of NeRFRenderer.forward
 // (src/render/nerf.py:251-303).  No CPU fallback: everything below launches CUDA kernels.
 #include <atomic>

@@ -1,4 +1,4 @@
-// Internal helpers shared by the libpnr_sm100 translation units.
+// Internal helpers shared by the libpnr_sm90 translation units.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -9,9 +9,9 @@
 // followed by one warp per point for pos-enc, projection and the 4-tap gather (latent scatter + d uv).
 // Row order inside a chunk is the forward SIMT engine's: row = local_point * NS + view.
 //
-// The GEMMs run on the tensor cores by default (split-bf16 tcgen05 GEMM, pnr_gemm_tc.cu); PNR_BWD_GEMM=simt selects
+// The GEMMs run on the tensor cores by default (split-bf16 wgmma GEMM, pnr_gemm_tc.cu); PNR_BWD_GEMM=simt selects
 // the fp32 FFMA SGEMM instead (the first, reference implementation of this path).
-// Validated on B200 against the oracle's formulas, the composed-torch path and the reference's own gradients
+// Validated on H100 against the oracle's formulas, the composed-torch path and the reference's own gradients
 // (tests/test_gpu_backward.py), compute-sanitizer memcheck clean.
 #include <stdlib.h>
 

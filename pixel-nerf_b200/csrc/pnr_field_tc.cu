@@ -1,15 +1,18 @@
 // Tensor engine: the conditioned MLP of pixelNeRF (ResnetFC d=512, 5 blocks, views averaged
 // before block 3; src/model/resnetfc.py:132-184) fused with point geometry, the latent gather,
 // the multi-view mean and the output activations (src/model/models.py:158-265) in ONE
-// persistent sm_100a kernel.  No [rows x 512] activation ever leaves the SM.
+// persistent sm_90a kernel.  No [rows x 512] activation ever leaves the SM.
 //
 // Design (DESIGN.md "tensor engine"):
-//  * A CTA PAIR (cluster of 2, tcgen05 cta_group::2, UMMA M=128 N=256 K=16) owns a tile of
-//    128 points (64 per CTA).  Per view it runs lin_in + 3 ResNet blocks on the (point, view)
-//    rows, sums the views through a per-thread-private scratch line, then runs blocks 3-4 and
+//  * A CTA owns 64 points of a 128-point tile (two CTAs per tile index).  Per view it runs lin_in + 3 ResNet blocks
+//    on the (point, view) rows, sums the views through a per-thread-private scratch line, then runs blocks 3-4 and
 //    lin_out on the averaged rows.
-//  * TMEM (512 columns) holds the two fp32 accumulators of a 64 x 512 row tile in the 2-CTA
-//    "2x2" layout: X (residual stream) in columns [0,256), H (hidden) in [256,512).
+//  * Two consumer warpgroups issue wgmma (m64n64k16, fp32 accumulators in registers).  Warpgroup g keeps features
+//    128q + 64g + [0, 64), q = 0..3, of the residual stream X in 128 registers per thread for the whole tile.  relu(X)
+//    is the A operand of fc_0 and lives in shared memory (64 x 512, fp16 hi/lo, 128 KB).  The hidden layer is never
+//    held in full: fc_0 and fc_1 are interleaved over 4 chunks of 128 hidden features, H_c = relu(X) W0_c^T (each
+//    warpgroup 64 features, 32 registers), relu(H_c) -> shared memory, X += relu(H_c) W1[:, c]^T.  Every weight tile
+//    holds 128 output rows; warpgroup g multiplies its rows [64g, 64g+64), so both warpgroups run the same steps.
 //  * Operands are error-compensated fp16 pairs: A = Ahi + Alo, W = Whi + Wlo (both splits exact
 //    to ~2^-22), D += Ahi*Whi + Alo*Whi + Ahi*Wlo with fp32 accumulation -- 3 tensor passes per
 //    algorithmic GEMM, the cheapest split that meets the 1e-4 RGB tolerance (SURVEY.md fact 8).
@@ -17,9 +20,10 @@
 //  * lin_z[i](latent) is NOT a per-sample GEMM: bilinear interpolation commutes with a linear
 //    layer, so pnr_project_latent builds P_i = lin_z[i](latent) (+ biases) once per encode()
 //    and the epilogue gathers 4 taps of P_i and adds them to the residual stream.
-//  * Warp roles per CTA: 8 worker warps (TMEM -> registers -> fp16 hi/lo -> 128B-swizzled smem A
-//    tiles, gathers, output), 1 MMA-issue warp (leader CTA; forwards barriers in the peer),
-//    1 weight-stream warp (cp.async.bulk of pre-swizzled 16 KB weight tiles, 5-slot ring).
+//  * Warp roles: 8 consumer warps (two warpgroups: geometry, wgmma, epilogues, ray finishing) and 1 weight-stream
+//    warp (cp.async.bulk of pre-swizzled 16 KB weight tiles in consumption order, 4-slot ring, mbarrier full/empty).
+//    ptxas allocates registers for 384 threads (168 per thread), so the 160 accumulator registers spill part of the
+//    epilogue state and serialize some wgmma: the kernel is correct, not yet tuned.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
@@ -39,41 +43,34 @@ namespace tc {
 
 constexpr int D = 512;
 constexpr int ROWS = 64;                 // rows (points) per CTA
-constexpr int TILE_POINTS = 128;         // per CTA pair
-constexpr int NWORKER_WARPS = 16;
-constexpr int WARP_MMA = NWORKER_WARPS;       // warp 16: MMA issue (leader) / slot forwarder (peer)
-constexpr int NTHREADS = (NWORKER_WARPS + 2) * 32;  // + warp 17: weight streamer
+constexpr int TILE_POINTS = 128;         // per tile index (two CTAs)
+constexpr int NCONSUMER_WARPS = 8;       // two warpgroups
+constexpr int NCONSUMERS = NCONSUMER_WARPS * 32;
+constexpr int NTHREADS = NCONSUMERS + 32;  // + warp 8: weight streamer
 constexpr int SLOT_BYTES = 16384;        // 128 weight rows x 64 k x fp16
-constexpr int NSLOTS = 6;
+constexpr int NSLOTS = 4;
 constexpr int A_CHUNK_BYTES = 16384;     // 64 rows x 64 k x fp16, hi then lo
 constexpr int A_BYTES = 8 * A_CHUNK_BYTES;
-constexpr int SLOTS_LIN_IN = 4;
-constexpr int SLOTS_FC = 32;
-constexpr int SLOTS_PER_RANK = SLOTS_LIN_IN + 10 * SLOTS_FC;  // 324
+constexpr int AH_BYTES = 2 * A_CHUNK_BYTES;  // relu(H_c): 128 hidden features
+constexpr int SLOTS_LIN_IN = 8;
+constexpr int SLOTS_BLOCK = 128;         // fc_0 and fc_1 of one ResNet block, interleaved by hidden chunk
+constexpr int SLOTS_TOTAL = SLOTS_LIN_IN + 5 * SLOTS_BLOCK;   // 648
 constexpr int HEADER_BYTES = 256;
-constexpr uint32_t X_COL = 0, H_COL = 256;
 
 // shared memory map (offsets from the 1024-aligned base)
 constexpr int SM_A = 0;
-constexpr int SM_B = SM_A + A_BYTES;                    // 131072
+constexpr int SM_AH = SM_A + A_BYTES;                   // 131072
+constexpr int SM_B = SM_AH + AH_BYTES;                  // 163840
 constexpr int SM_GEO = SM_B + NSLOTS * SLOT_BYTES;      // [64][8] words: 4 tap offsets + 4 bilinear weights per row
-constexpr int SM_PART = SM_A;                           // lin_out partials [64][8][4] floats alias A chunk 0 (free at tile end)
+constexpr int SM_PART = SM_A;                           // lin_out partials [64][2][4] floats alias A chunk 0 (free at tile end)
 constexpr int SM_BAR = SM_GEO + ROWS * 8 * 4;
-constexpr int SM_TOTAL = SM_BAR + 512;
-constexpr int SMEM_BYTES = SM_TOTAL;
-
-// barrier indices (8 bytes each)
-constexpr int BAR_B_FULL = 0;                 // [NSLOTS]
-constexpr int BAR_B_PEER = BAR_B_FULL + NSLOTS;   // [NSLOTS] (leader only)
-constexpr int BAR_B_EMPTY = BAR_B_PEER + NSLOTS;  // [NSLOTS]
-constexpr int BAR_A_FULL = BAR_B_EMPTY + NSLOTS;  // [8]
-constexpr int BAR_A_FREE = BAR_A_FULL + 8;         // [8] chunk consumed by the MMA of the current fc layer
-constexpr int BAR_F_FULL = BAR_A_FREE + 8;
-constexpr int BAR_ACC = BAR_F_FULL + 1;             // [2] accumulator block 0 / block 1 ready
-constexpr int BAR_COUNT = BAR_ACC + 2;
-constexpr int SM_TMEM_PTR = SM_BAR + BAR_COUNT * 8;
-constexpr int SM_NLIST = SM_TMEM_PTR + 8;     // fused render: number of rays this CTA completed in the current pass
-constexpr int FLUSH_SCRATCH_BYTES = A_BYTES / NWORKER_WARPS;   // per-warp scratch (cdf + merged samples) in the idle A buffer
+constexpr int BAR_FULL = 0;                             // [NSLOTS]
+constexpr int BAR_EMPTY = BAR_FULL + NSLOTS;            // [NSLOTS]
+constexpr int BAR_COUNT = BAR_EMPTY + NSLOTS;
+constexpr int SM_NLIST = SM_BAR + BAR_COUNT * 8;        // fused render: number of rays this CTA completed in the current pass
+constexpr int SMEM_BYTES = SM_NLIST + 16;
+static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
+constexpr int FLUSH_SCRATCH_BYTES = A_BYTES / NCONSUMER_WARPS;   // per-warp scratch (cdf + merged samples) in the idle A buffer
 
 
 // One evaluation pass of the field: the coarse or the fine MLP over a set of points.
@@ -119,20 +116,10 @@ struct Params {
 };
 
 using namespace tcptx;
-constexpr uint32_t IDESC = IDESC_M128_N256;
 
-enum { MODE_GATHER = 0, MODE_BIAS_WB = 1, MODE_HIDDEN = 2, MODE_COMBINE = 3, MODE_OUT = 4 };
+enum { MODE_GATHER = 0, MODE_BIAS_WB = 1, MODE_COMBINE = 2, MODE_OUT = 3 };
 
-struct WorkerCtx {
-  uint8_t* smem;
-  uint32_t smem_u;      // shared::cta address of the smem base
-  uint32_t tmem;        // base tmem address incl. this warp's lane quarter
-  uint32_t bar_base;    // smem address of the barrier array
-  int lane, s, m, n_hi;
-  float w_scale, w_inv;
-  uint64_t l2_keep;     // createpolicy evict_last (view-sum scratch)
-  long long* t_acc;     // cycles spent waiting for the accumulator barrier
-};
+__device__ __forceinline__ void workers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 __device__ __forceinline__ void st_evict_last(float* q, float v, uint64_t pol) {
   asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(q), "f"(v), "l"(pol) : "memory");
@@ -142,41 +129,8 @@ __device__ __forceinline__ float ld_evict_last(const float* q, uint64_t pol) {
   asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(q), "l"(pol) : "memory");
   return v;
 }
-
-// A worker thread owns row m and 8 "steps" of 8 features per layer:
-//   step i -> (b = i>>2 MMA block, c = (i>>1)&1 chunk half, h = i&1): features b*256 + n_hi*128 + c*64 + s*16 + h*8 .. +8
-// i.e. the 16 warps sweep the k-chunks of the next layer in 4 waves (2 chunks per wave), so the MMA warp can
-// start after a quarter of the epilogue.  Chunk j = 4b + 2 n_hi + c, column offset inside the chunk s*16 + h*8.
-__device__ __forceinline__ int step_feature(const WorkerCtx& c, int i) {
-  return (i >> 2) * 256 + c.n_hi * 128 + ((i >> 1) & 1) * 64 + c.s * 16 + (i & 1) * 8;
-}
-__device__ __forceinline__ uint32_t step_tmem_col(const WorkerCtx& c, int i) {
-  return (uint32_t)((i >> 2) * 128 + ((i >> 1) & 1) * 64 + c.s * 16 + (i & 1) * 8);
-}
-
-// TMEM load of 8 columns WITHOUT waiting: the registers are valid only after tmem_ld_wait8 (which carries them as
-// in/out operands so that no use can be scheduled ahead of the wait).
-__device__ __forceinline__ void tmem_ld8_issue(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait8(uint32_t* r) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7])
-               :
-               : "memory");
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t saddr, uint4 v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ float4 ld_shared_f4(uint32_t saddr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_shared_f4(uint32_t saddr, float4 v) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+__device__ __forceinline__ void st_shared_u32(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
 }
 // relu(y0), relu(y1) -> packed fp16 hi pair and lo pair (error-compensated split); F2FP packs two values per
 // instruction on the fast pipe and saturates instead of producing inf.
@@ -186,219 +140,264 @@ __device__ __forceinline__ void split_relu2(float y0, float y1, uint32_t& hi, ui
   const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(a1 - hf.y), "f"(a0 - hf.x));
 }
-
-// Where the 16-byte hi unit of (row m, features [8u, 8u+8) of k-chunk j) lives in the A buffer; the lo unit is
-// 8192 bytes further.  The SAME two slots first hold the staged gather values G[m][8u..8u+3] and G[m][8u+4..8u+7].
-__device__ __forceinline__ uint32_t a_unit_offset(int j, int m, int u) {
-  return (uint32_t)(SM_A + j * A_CHUNK_BYTES + m * 128 + ((u ^ (m & 7)) * 16));
+// byte offset of the 16-bit pair (row m, k columns [k, k+2) of the 64-wide chunk), k even, in a 128B-swizzled tile
+__device__ __forceinline__ uint32_t swz(int m, int k) {
+  return (uint32_t)(m * 128 + ((((k >> 3) ^ (m & 7))) << 4) + (k & 7) * 2);
 }
 
-// Coalesced gather of the projected-latent map: G[row][:] = sum_k w_k * P_i[tap_k(row)][:].  A warp-load covers two
-// rows x 64 features with lane = feature (2 x 256 contiguous bytes per tap instead of the 32 scattered lines a
-// lane-per-row gather costs); the result is parked in the (free) A-operand buffer, in exactly the two 16-byte slots
-// that the thread owning (row, 8 features) overwrites with its fp16 hi/lo units later.
-// One k-chunk (64 features) of all 64 rows; staged chunk by chunk so that it can run while the tensor core is still
-// consuming the rest of the A buffer.
-__device__ __forceinline__ void stage_gather_chunk(uint8_t* smem, uint32_t smem_u, const float* __restrict__ proj_i,
-                                                   int j, int warp, int lane) {
-  const uint32_t* geo_all = reinterpret_cast<const uint32_t*>(smem + SM_GEO);
-  const int sub = lane >> 4, l16 = lane & 15;
-  // both row pairs of this warp: all 8 tap loads are issued before the first use (one L2 round trip, not two)
-  float4 t[2][4];
-#pragma unroll
-  for (int it = 0; it < 2; ++it) {
-    const uint32_t* geo = geo_all + (warp * 4 + it * 2 + sub) * 8;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) t[it][k] = __ldg(reinterpret_cast<const float4*>(proj_i + geo[k] + j * 64) + l16);
+// Weight ring: the streamer fills the slots in exactly the order the consumers use them, and every step of a
+// consumer warpgroup takes two consecutive slots (W_hi, W_lo of one 128-row x 64-k tile).  A step's slots are
+// released once the wgmma that read them has completed (one step later: wait_group 1).
+struct Ring {
+  uint32_t bar_base, b_base;
+  uint32_t seq;      // slot sequence number of the next step
+  uint32_t pend;     // first slot of the step still in flight (valid if has_pend)
+  bool has_pend;
+  int lane;
+  int* status;
+  __device__ __forceinline__ uint32_t slot_addr(uint32_t s) const { return b_base + (s % NSLOTS) * SLOT_BYTES; }
+  __device__ __forceinline__ void acquire() {
+    for (uint32_t s = seq; s < seq + 2; ++s)
+      mbar_wait(bar_base + (BAR_FULL + s % NSLOTS) * 8, (s / NSLOTS) & 1, status, 200 + (int)(s % NSLOTS));
   }
+  __device__ __forceinline__ void release(uint32_t s) {
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(bar_base + (BAR_EMPTY + s % NSLOTS) * 8);
+      mbar_arrive(bar_base + (BAR_EMPTY + (s + 1) % NSLOTS) * 8);
+    }
+  }
+  // after the step's wgmma are issued: commit them as one group, retire the previous step
+  __device__ __forceinline__ void issued() {
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (has_pend) release(pend);
+    pend = seq;
+    has_pend = true;
+    seq += 2;
+  }
+  __device__ __forceinline__ void drain() {
+    wgmma_wait<0>();
+    if (has_pend) release(pend);
+    has_pend = false;
+  }
+};
+
+// acc (+)= A[64 x 16 KSTEPS] * W^T over one step: Ahi*Whi + Alo*Whi + Ahi*Wlo
+template <int KSTEPS>
+__device__ __forceinline__ void mma3(float* acc, uint64_t a_hi, uint64_t b_hi, uint64_t b_lo, bool zero) {
+  const uint64_t a_lo = a_hi + (8192 >> 4);
 #pragma unroll
-  for (int it = 0; it < 2; ++it) {
-    const int row = warp * 4 + it * 2 + sub;
-    const uint32_t* geo = geo_all + row * 8;
-    const float w0 = __uint_as_float(geo[4]), w1 = __uint_as_float(geo[5]), w2 = __uint_as_float(geo[6]),
-                w3 = __uint_as_float(geo[7]);
-    float4 g;
-    g.x = ((t[it][0].x * w0 + t[it][1].x * w1) + t[it][2].x * w2) + t[it][3].x * w3;
-    g.y = ((t[it][0].y * w0 + t[it][1].y * w1) + t[it][2].y * w2) + t[it][3].y * w3;
-    g.z = ((t[it][0].z * w0 + t[it][1].z * w1) + t[it][2].z * w2) + t[it][3].z * w3;
-    g.w = ((t[it][0].w * w0 + t[it][1].w * w1) + t[it][2].w * w2) + t[it][3].w * w3;
-    st_shared_f4(smem_u + a_unit_offset(j, row, l16 >> 1) + ((l16 & 1) ? 8192u : 0u), g);
+  for (int kk = 0; kk < KSTEPS; ++kk) {
+    wgmma_m64n64_f16(acc, a_hi + 2 * kk, b_hi + 2 * kk, (zero && kk == 0) ? 0u : 1u);
+    wgmma_m64n64_f16(acc, a_lo + 2 * kk, b_hi + 2 * kk, 1u);
+    wgmma_m64n64_f16(acc, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
   }
 }
-// two chunks at once (the two chunks of an epilogue wave): 16 tap loads in flight per lane
-__device__ __forceinline__ void stage_gather_pair(uint8_t* smem, uint32_t smem_u, const float* __restrict__ proj_i,
-                                                  int j0, int j1, int warp, int lane) {
-  const uint32_t* geo_all = reinterpret_cast<const uint32_t*>(smem + SM_GEO);
-  const int sub = lane >> 4, l16 = lane & 15;
-  float4 t[4][4];
+
+struct Cons {
+  uint32_t smem_u;
+  int tid, wg, lane;
+  int r0, c0;           // row of accumulator elements with ((i >> 1) & 1) == 0; column offset 2 (lane % 4)
+  float w_scale, w_inv;
+  uint64_t l2_keep;     // createpolicy evict_last (view-sum scratch)
+};
+
+// lin_in (K = 42 -> 48) and the fc_1 steps over one 64-wide k-chunk: 4 steps of 128 output rows (N block q);
+// warpgroup g accumulates rows [64g, 64g+64) of each into x[q].
+template <int KSTEPS>
+__device__ __forceinline__ void wide_steps(Ring& rg, const Cons& c, float (&x)[4][32], uint64_t a_hi, bool zero) {
+  const uint64_t desc0 = make_desc(0);
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    const uint32_t* geo = geo_all + (warp * 4 + (q & 1) * 2 + sub) * 8;
-    const int j = (q >> 1) ? j1 : j0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) t[q][k] = __ldg(reinterpret_cast<const float4*>(proj_i + geo[k] + j * 64) + l16);
-  }
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int row = warp * 4 + (q & 1) * 2 + sub;
-    const int j = (q >> 1) ? j1 : j0;
-    const uint32_t* geo = geo_all + row * 8;
-    const float w0 = __uint_as_float(geo[4]), w1 = __uint_as_float(geo[5]), w2 = __uint_as_float(geo[6]),
-                w3 = __uint_as_float(geo[7]);
-    float4 g;
-    g.x = ((t[q][0].x * w0 + t[q][1].x * w1) + t[q][2].x * w2) + t[q][3].x * w3;
-    g.y = ((t[q][0].y * w0 + t[q][1].y * w1) + t[q][2].y * w2) + t[q][3].y * w3;
-    g.z = ((t[q][0].z * w0 + t[q][1].z * w1) + t[q][2].z * w2) + t[q][3].z * w3;
-    g.w = ((t[q][0].w * w0 + t[q][1].w * w1) + t[q][2].w * w2) + t[q][3].w * w3;
-    st_shared_f4(smem_u + a_unit_offset(j, row, l16 >> 1) + ((l16 & 1) ? 8192u : 0u), g);
+    rg.acquire();
+    const uint64_t b_hi = desc0 + ((rg.slot_addr(rg.seq) + c.wg * 8192) >> 4);
+    const uint64_t b_lo = desc0 + ((rg.slot_addr(rg.seq + 1) + c.wg * 8192) >> 4);
+    fence_acc<32>(x[q]);
+    wgmma_fence();
+    mma3<KSTEPS>(x[q], a_hi, b_hi, b_lo, zero);
+    rg.issued();
   }
 }
 
-// One epilogue pass over this thread's 64 features of one layer, in two halves of 4 steps: the MMA warp computes a
-// layer feature-block by feature-block (b = 0: features 0..255, then b = 1), so half 0 (steps 0..3, k-chunks 0..3 of
-// the next layer) runs after BAR_ACC+0 while the tensor core is still busy with block 1, and half 1 after BAR_ACC+1.
-//   gate / free_par : the layer that is still running also reads the A buffer; chunk j may only be overwritten once
-//                     its block-1 pass has consumed it (a_free[j], phase free_par).
-// TMEM loads and bias loads of the next step are issued before the current step is processed; MODE_GATHER reads the
-// staged gather values back from shared memory (staged here as the chunks are released, when gated).
+// fc_0 and fc_1 of one ResNet block: X += W1 relu(W0 relu(X) + b0) (the fc_1 bias is added by the caller's epilogue).
+__device__ __forceinline__ void fc_block(Ring& rg, const Cons& c, float (&x)[4][32], const float* __restrict__ b0,
+                                         const int* status) {
+  const uint64_t desc0 = make_desc(0);
+  float h[32];
+#pragma unroll 1
+  for (int hc = 0; hc < 4; ++hc) {
+    // ---- H_c = relu(X) W0[128 hc + 64 g, +64)^T over K = 512 ----
+#pragma unroll 1
+    for (int j = 0; j < 8; ++j) {
+      rg.acquire();
+      const uint64_t a_hi = desc0 + ((c.smem_u + SM_A + j * A_CHUNK_BYTES) >> 4);
+      const uint64_t b_hi = desc0 + ((rg.slot_addr(rg.seq) + c.wg * 8192) >> 4);
+      const uint64_t b_lo = desc0 + ((rg.slot_addr(rg.seq + 1) + c.wg * 8192) >> 4);
+      fence_acc<32>(h);
+      wgmma_fence();
+      mma3<4>(h, a_hi, b_hi, b_lo, j == 0);
+      rg.issued();
+    }
+    rg.drain();
+    fence_acc<32>(h);
+    workers_sync();   // both warpgroups are done with relu(H_{c-1})
+    // ---- relu(H_c + b0) -> fp16 hi/lo chunk g of the relu(H) buffer ----
+    const float* bc = b0 + hc * 128 + c.wg * 64;
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int col = 8 * (i >> 2) + c.c0, m = c.r0 + 8 * ((i >> 1) & 1);
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(bc + col));
+      uint32_t hi, lo;
+      split_relu2(h[i] * c.w_inv + bb.x, h[i + 1] * c.w_inv + bb.y, hi, lo);
+      const uint32_t a = c.smem_u + SM_AH + c.wg * A_CHUNK_BYTES + swz(m, col);
+      st_shared_u32(a, hi);
+      st_shared_u32(a + 8192, lo);
+    }
+    fence_proxy_async();
+    workers_sync();
+    // ---- X += relu(H_c) W1[:, 128 hc, +128)^T ----
+#pragma unroll 1
+    for (int jj = 0; jj < 2; ++jj)
+      wide_steps<4>(rg, c, x, desc0 + ((c.smem_u + SM_AH + jj * A_CHUNK_BYTES) >> 4), false);
+  }
+}
+
+// Coalesced gather of the projected-latent map into the (idle) A buffer: G[row][:] = sum_k w_k * P_i[tap_k(row)][:].
+// A warp-load covers two rows x 64 features with lane = feature (2 x 256 contiguous bytes per tap instead of the 32
+// scattered lines a lane-per-row gather costs).  G[m][8u..8u+3] and G[m][8u+4..8u+7] of a k-chunk are parked in
+// exactly the two 16-byte units (hi, lo) that the fp16 split of those 8 features overwrites later.
+__device__ __forceinline__ void stage_gather(uint32_t smem_u, const float* __restrict__ proj_i, int warp, int lane) {
+  const int sub = lane >> 4, l16 = lane & 15;
+#pragma unroll 1
+  for (int j = 0; j < 8; ++j) {
+    float4 t[4][4];
+    uint32_t geo[4][4];
+    float w[4][4];
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+      const uint32_t ga = smem_u + SM_GEO + (warp * 8 + it * 2 + sub) * 32;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        uint32_t wb;
+        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(geo[it][k]) : "r"(ga + 4 * k));
+        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(wb) : "r"(ga + 16 + 4 * k));
+        w[it][k] = __uint_as_float(wb);
+      }
+    }
+    // all 16 tap loads are issued before the first use (one L2 round trip)
+#pragma unroll
+    for (int it = 0; it < 4; ++it)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) t[it][k] = __ldg(reinterpret_cast<const float4*>(proj_i + geo[it][k] + j * 64) + l16);
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+      const int row = warp * 8 + it * 2 + sub;
+      float4 g;
+      g.x = ((t[it][0].x * w[it][0] + t[it][1].x * w[it][1]) + t[it][2].x * w[it][2]) + t[it][3].x * w[it][3];
+      g.y = ((t[it][0].y * w[it][0] + t[it][1].y * w[it][1]) + t[it][2].y * w[it][2]) + t[it][3].y * w[it][3];
+      g.z = ((t[it][0].z * w[it][0] + t[it][1].z * w[it][1]) + t[it][2].z * w[it][2]) + t[it][3].z * w[it][3];
+      g.w = ((t[it][0].w * w[it][0] + t[it][1].w * w[it][1]) + t[it][2].w * w[it][2]) + t[it][3].w * w[it][3];
+      const uint32_t a = smem_u + SM_A + j * A_CHUNK_BYTES + swz(row, (l16 >> 1) * 8) + ((l16 & 1) ? 8192u : 0u);
+      asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(g.x), "f"(g.y), "f"(g.z), "f"(g.w) : "memory");
+    }
+  }
+}
+
+// Epilogue of a layer that ends on the residual stream: y = X / s + (gathered projected latent | bias), then
+//   GATHER / BIAS_WB: X = y, relu(y) -> fp16 hi/lo A operand;   COMBINE: view sum (mean after the last view), ditto
+//   OUT: lin_out partial sums of relu(y) into out_part.
 template <int MODE>
-__device__ __forceinline__ void epilogue(const WorkerCtx& c, const Params& p, const float* __restrict__ lin_out_w, uint32_t acc_col,
-                                         const float* __restrict__ bias, const float* __restrict__ proj_i,
-                                         int view, float* __restrict__ scratch, float* out_part, uint32_t acc_phase,
-                                         bool gate, uint32_t free_par, int warp, int tag) {
-  float4 bb[2][2];
-  uint32_t raw[8];
-  if (MODE != MODE_GATHER) {
-    bb[0][0] = __ldg(reinterpret_cast<const float4*>(bias + step_feature(c, 0)));
-    bb[0][1] = __ldg(reinterpret_cast<const float4*>(bias + step_feature(c, 0)) + 1);
-  }
-  float o0 = 0.f, o1 = 0.f, o2 = 0.f, o3 = 0.f;
-  const int NS = p.sc.NS;
+__device__ __forceinline__ void epilogue_x(Ring& rg, const Cons& c, float (&x)[4][32], const float* __restrict__ bias,
+                                           const float* __restrict__ proj_i, const float* __restrict__ lin_out_w,
+                                           int view, int NS, float* __restrict__ scratch, float* out_part) {
+  rg.drain();
+#pragma unroll
+  for (int q = 0; q < 4; ++q) fence_acc<32>(x[q]);
+  workers_sync();   // every warpgroup's wgmma reading the A buffer are complete
   const bool produce = (MODE != MODE_OUT) && !(MODE == MODE_COMBINE && view != NS - 1);
+  if (MODE == MODE_GATHER) {
+    stage_gather(c.smem_u, proj_i, c.tid >> 5, c.lane);
+    workers_sync();
+  }
+  float o[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
 #pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    if (MODE == MODE_GATHER && gate && half == 1) {
-      // the tail of the running layer releases chunks 4, 6, 5, 7: stage them before its accumulator barrier
-      mbar_wait(c.bar_base + (BAR_A_FREE + 4) * 8, free_par, p.status, 144);
-      mbar_wait(c.bar_base + (BAR_A_FREE + 6) * 8, free_par, p.status, 146);
-      stage_gather_pair(c.smem, c.smem_u, proj_i, 4, 6, warp, c.lane);
-      mbar_wait(c.bar_base + (BAR_A_FREE + 5) * 8, free_par, p.status, 145);
-      mbar_wait(c.bar_base + (BAR_A_FREE + 7) * 8, free_par, p.status, 147);
-      stage_gather_pair(c.smem, c.smem_u, proj_i, 5, 7, warp, c.lane);
-      workers_sync();
-    }
-    mbar_wait_timed(c.bar_base + (BAR_ACC + half) * 8, acc_phase, p.status, tag + half, *c.t_acc);
-    tc_fence_after();
-    if (MODE == MODE_GATHER && !gate && half == 0) {
-      // block 0 of a view: chunks 1..7 were staged while lin_in ran; chunk 0 holds lin_in's operand, which BOTH of its
-      // passes read, so wait for the second accumulator barrier as well before overwriting it
-      mbar_wait_timed(c.bar_base + (BAR_ACC + 1) * 8, acc_phase, p.status, tag + 1, *c.t_acc);
-      stage_gather_chunk(c.smem, c.smem_u, proj_i, 0, warp, c.lane);
-      workers_sync();
-    }
-    tmem_ld8_issue(c.tmem + acc_col + step_tmem_col(c, 4 * half), raw);
+  for (int q = 0; q < 4; ++q) {
 #pragma unroll
-    for (int ii = 0; ii < 4; ++ii) {
-      const int i = 4 * half + ii;
-      const int n0 = step_feature(c, i);
-      const uint32_t col = step_tmem_col(c, i);
-      const int j = 4 * (i >> 2) + 2 * c.n_hi + ((i >> 1) & 1);
-      const uint32_t unit = c.smem_u + a_unit_offset(j, c.m, 2 * c.s + (i & 1));
-      if ((i & 1) == 0 && gate) {
-        if (MODE == MODE_GATHER) {
-          if (half == 0) {
-            const int j0 = ((i >> 1) & 1), j1 = j0 + 2;
-            mbar_wait(c.bar_base + (BAR_A_FREE + j0) * 8, free_par, p.status, 140 + j0);
-            mbar_wait(c.bar_base + (BAR_A_FREE + j1) * 8, free_par, p.status, 140 + j1);
-            stage_gather_pair(c.smem, c.smem_u, proj_i, j0, j1, warp, c.lane);
-            workers_sync();
-          }
-        } else if (produce) {
-          mbar_wait(c.bar_base + (BAR_A_FREE + j) * 8, free_par, p.status, 150 + j);
-        }
-      }
-      float y[8];
-      tmem_ld_wait8(raw);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) y[e] = __uint_as_float(raw[e]) * c.w_inv;
-      if (ii + 1 < 4) tmem_ld8_issue(c.tmem + acc_col + step_tmem_col(c, i + 1), raw);
-      if (MODE != MODE_GATHER && i + 1 < 8) {
-        bb[(i + 1) & 1][0] = __ldg(reinterpret_cast<const float4*>(bias + step_feature(c, i + 1)));
-        bb[(i + 1) & 1][1] = __ldg(reinterpret_cast<const float4*>(bias + step_feature(c, i + 1)) + 1);
-      }
+    for (int i = 0; i < 32; i += 2) {
+      const int r = (i >> 1) & 1, m = c.r0 + 8 * r;
+      const int f = 128 * q + 64 * c.wg + 8 * (i >> 2) + c.c0;
+      float y0 = x[q][i] * c.w_inv, y1 = x[q][i + 1] * c.w_inv;
       if (MODE == MODE_GATHER) {
-        const float4 g0 = ld_shared_f4(unit), g1 = ld_shared_f4(unit + 8192);
-        y[0] += g0.x; y[1] += g0.y; y[2] += g0.z; y[3] += g0.w;
-        y[4] += g1.x; y[5] += g1.y; y[6] += g1.z; y[7] += g1.w;
+        // the staged G pair of (m, f, f+1); the quad that shares its 16-byte units reads them all before any writes
+        const uint32_t a = c.smem_u + SM_A + (f >> 6) * A_CHUNK_BYTES + swz(m, (f & 63) & ~7) + (c.c0 >= 4 ? 8192u : 0u) +
+                           (c.c0 & 3) * 4;
+        float2 g;
+        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(g.x), "=f"(g.y) : "r"(a) : "memory");
+        __syncwarp();
+        y0 += g.x;
+        y1 += g.y;
       } else {
-        const float4 b0 = bb[i & 1][0], b1 = bb[i & 1][1];
-        y[0] += b0.x; y[1] += b0.y; y[2] += b0.z; y[3] += b0.w;
-        y[4] += b1.x; y[5] += b1.y; y[6] += b1.z; y[7] += b1.w;
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + f));
+        y0 += bb.x;
+        y1 += bb.y;
       }
       if (MODE == MODE_COMBINE && NS > 1) {
-        // view-sum scratch: 19 MB that every CTA rewrites and re-reads NS-1 times per tile.  Together with the two
-        // MLPs' projected maps and weight images the L2 working set (~140 MB at C2) exceeds the 126 MB L2, and plain
-        // LRU then evicts DIRTY scratch lines to DRAM; evict_last keeps the small hot scratch resident instead
-        float* sp = scratch + (size_t)n0 * ROWS + c.m;
+        // view-sum scratch (thread-private, coalesced): 128 KB per CTA that every CTA rewrites and re-reads NS-1
+        // times per tile.  With both MLPs' projected maps and weight images streaming through the 50 MB L2, plain
+        // LRU would evict DIRTY scratch lines to DRAM; evict_last keeps the small hot scratch resident instead
+        float* sp = scratch + (size_t)((q * 32 + i) * NCONSUMERS + c.tid);
         if (view == 0) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) st_evict_last(sp + e * ROWS, y[e], c.l2_keep);
+          st_evict_last(sp, y0, c.l2_keep);
+          st_evict_last(sp + NCONSUMERS, y1, c.l2_keep);
         } else {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) y[e] = ld_evict_last(sp + e * ROWS, c.l2_keep) + y[e];
+          y0 = ld_evict_last(sp, c.l2_keep) + y0;
+          y1 = ld_evict_last(sp + NCONSUMERS, c.l2_keep) + y1;
           if (view < NS - 1) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) st_evict_last(sp + e * ROWS, y[e], c.l2_keep);
+            st_evict_last(sp, y0, c.l2_keep);
+            st_evict_last(sp + NCONSUMERS, y1, c.l2_keep);
           } else {
             const float ns = (float)NS;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) y[e] = y[e] / ns;
+            y0 = y0 / ns;
+            y1 = y1 / ns;
           }
         }
       }
-      if (MODE == MODE_GATHER || MODE == MODE_BIAS_WB || (MODE == MODE_COMBINE && produce)) {
-        float z[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) z[e] = y[e] * c.w_scale;
-        tmem_st8(c.tmem + X_COL + col, z);
-      }
       if (MODE == MODE_OUT) {
-        const float* W = lin_out_w + n0;
+        const float a0 = fmaxf(y0, 0.f), a1 = fmaxf(y1, 0.f);
 #pragma unroll
-        for (int e4 = 0; e4 < 2; ++e4) {
-          const float4 w0 = __ldg(reinterpret_cast<const float4*>(W + 0 * D) + e4);
-          const float4 w1 = __ldg(reinterpret_cast<const float4*>(W + 1 * D) + e4);
-          const float4 w2 = __ldg(reinterpret_cast<const float4*>(W + 2 * D) + e4);
-          const float4 w3 = __ldg(reinterpret_cast<const float4*>(W + 3 * D) + e4);
-          const float a0 = fmaxf(y[4 * e4 + 0], 0.f), a1 = fmaxf(y[4 * e4 + 1], 0.f);
-          const float a2 = fmaxf(y[4 * e4 + 2], 0.f), a3 = fmaxf(y[4 * e4 + 3], 0.f);
-          o0 = fmaf(a3, w0.w, fmaf(a2, w0.z, fmaf(a1, w0.y, fmaf(a0, w0.x, o0))));
-          o1 = fmaf(a3, w1.w, fmaf(a2, w1.z, fmaf(a1, w1.y, fmaf(a0, w1.x, o1))));
-          o2 = fmaf(a3, w2.w, fmaf(a2, w2.z, fmaf(a1, w2.y, fmaf(a0, w2.x, o2))));
-          o3 = fmaf(a3, w3.w, fmaf(a2, w3.z, fmaf(a1, w3.y, fmaf(a0, w3.x, o3))));
+        for (int k = 0; k < 4; ++k) {
+          const float2 w = __ldg(reinterpret_cast<const float2*>(lin_out_w + k * D + f));
+          o[r][k] = fmaf(a1, w.y, fmaf(a0, w.x, o[r][k]));
         }
       } else if (produce) {
-        uint4 vhi, vlo;
-        split_relu2(y[0], y[1], vhi.x, vlo.x);
-        split_relu2(y[2], y[3], vhi.y, vlo.y);
-        split_relu2(y[4], y[5], vhi.z, vlo.z);
-        split_relu2(y[6], y[7], vhi.w, vlo.w);
-        st_shared_v4(unit, vhi);
-        st_shared_v4(unit + 8192, vlo);
-        if (i & 1) {
-          fence_proxy_async();
-          if (MODE != MODE_HIDDEN) tmem_wait_st();
-          tc_fence_before();
-          __syncwarp();
-          if (c.lane == 0) mbar_arrive_cta(c.bar_base + (BAR_A_FULL + j) * 8, 0);
-        }
+        x[q][i] = y0 * c.w_scale;
+        x[q][i + 1] = y1 * c.w_scale;
+        uint32_t hi, lo;
+        split_relu2(y0, y1, hi, lo);
+        const uint32_t a = c.smem_u + SM_A + (f >> 6) * A_CHUNK_BYTES + swz(m, f & 63);
+        st_shared_u32(a, hi);
+        st_shared_u32(a + 8192, lo);
       }
     }
   }
   if (MODE == MODE_OUT) {
-    float4* dst = reinterpret_cast<float4*>(out_part) + c.m * 8 + (c.n_hi * 4 + c.s);
-    *dst = make_float4(o0, o1, o2, o3);
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        o[r][k] += __shfl_xor_sync(0xffffffffu, o[r][k], 1);
+        o[r][k] += __shfl_xor_sync(0xffffffffu, o[r][k], 2);
+      }
+    if ((c.lane & 3) == 0) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r)
+        reinterpret_cast<float4*>(out_part)[(c.r0 + 8 * r) * 2 + c.wg] = make_float4(o[r][0], o[r][1], o[r][2], o[r][3]);
+    }
+  } else if (produce) {
+    fence_proxy_async();
   }
+  workers_sync();
 }
 
 // Loads of values that OTHER CTAs wrote during this launch (field values, samples): L2, never a stale L1 line.
@@ -460,68 +459,52 @@ __device__ __forceinline__ void finish_ray(const Params& p, int ps, int64_t ray,
   }
 }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant__ Params p) {
+__global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant__ Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
+  const int rank = blockIdx.x & 1;        // which 64 points of the 128-point tile
   const int pair = blockIdx.x >> 1;
   const int n_pairs = gridDim.x >> 1;
   const uint32_t bar_base = smem_u32(smem + SM_BAR);
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + SM_TMEM_PTR);
   int* n_list = reinterpret_cast<int*>(smem + SM_NLIST);
   const int NS = p.sc.NS;
   const bool render = p.rn.rays != nullptr;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < NSLOTS; ++i) {
-      mbar_init(bar_base + (BAR_B_FULL + i) * 8, 1);
-      mbar_init(bar_base + (BAR_B_PEER + i) * 8, 1);
-      mbar_init(bar_base + (BAR_B_EMPTY + i) * 8, 1);
+      mbar_init(bar_base + (BAR_FULL + i) * 8, 1);
+      mbar_init(bar_base + (BAR_EMPTY + i) * 8, NCONSUMER_WARPS);
     }
-    for (int i = 0; i < 8; ++i) {
-      mbar_init(bar_base + (BAR_A_FULL + i) * 8, 16);  // 8 warps x 2 CTAs per chunk
-      mbar_init(bar_base + (BAR_A_FREE + i) * 8, 1);
-    }
-    mbar_init(bar_base + BAR_F_FULL * 8, 2 * NWORKER_WARPS);
-    mbar_init(bar_base + (BAR_ACC + 0) * 8, 1);
-    mbar_init(bar_base + (BAR_ACC + 1) * 8, 1);
     *n_list = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == WARP_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   const size_t map_stride = (size_t)p.sc.SB * NS * p.sc.Hl * p.sc.Wl * D;
 
-  if (warp < NWORKER_WARPS) {
-    // =============================== worker warps ===============================
-    WorkerCtx c;
-    c.smem = smem;
+  if (warp < NCONSUMER_WARPS) {
+    // =============================== consumer warpgroups ===============================
+    Cons c;
     c.smem_u = smem_u32(smem);
+    c.tid = threadIdx.x;
+    c.wg = threadIdx.x >> 7;
     c.lane = lane;
-    const int q = warp & 3;          // TMEM lane quarter this warp may access
-    c.s = warp >> 2;                 // 0..3: which 16 columns of every chunk
-    c.m = 32 * (q & 1) + lane;       // row of the CTA's 64-row tile
-    c.n_hi = q >> 1;                 // which 128 features of a 256-wide MMA block live in these lanes
-    c.tmem = tmem_base + ((uint32_t)(32 * q) << 16);
-    c.bar_base = bar_base;
+    c.r0 = 16 * (warp & 3) + (lane >> 2);
+    c.c0 = 2 * (lane & 3);
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(c.l2_keep));
-    long long t_acc = 0;
-    c.t_acc = &t_acc;
+    Ring rg;
+    rg.bar_base = bar_base;
+    rg.b_base = smem_u32(smem + SM_B);
+    rg.seq = 0;
+    rg.pend = 0;
+    rg.has_pend = false;
+    rg.lane = lane;
+    rg.status = p.status;
+    float x[4][32];
     float* scratch = p.scratch + (size_t)blockIdx.x * D * ROWS;
     float* out_part = reinterpret_cast<float*>(smem + SM_PART);
-    uint32_t acc_phase = 0;
-    uint32_t fc_idx = 0;   // number of fc layers whose A operand has been produced so far
     const int grow = threadIdx.x & 63;   // row handled in the geometry stage
-    const int gsub = threadIdx.x >> 6;   // 0..7: which 6 of the 48 input channels
+    const int gsub = threadIdx.x >> 6;   // 0..3: which 12 of the 48 input channels
+    const uint64_t a0_desc = make_desc(c.smem_u + SM_A);   // A chunk 0: the lin_in operand
 
     for (int ps = 0; ps < p.npass; ++ps) {
       const Pass& P = p.pass[ps];
@@ -531,7 +514,7 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1) k_field
         const int64_t pt_raw = tile * TILE_POINTS + rank * ROWS + grow;
         const int64_t pt = pt_raw < P.total_points ? pt_raw : P.total_points - 1;
         const int sb = (int)(pt / P.P);
-        float x[3], d[3];
+        float xp[3], d[3];
         if (render) {
           // the sample depth is produced here: stratified draw (coarse, nerf.py:98-113) or the merged fine sample that
           // the CTA which finished the ray's coarse pass has written
@@ -544,8 +527,8 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1) k_field
             if (gsub == 0 && pt_raw < P.total_points) p.rn.zc[pt] = zz;
           } else {
             // ONE poller per ray segment of this CTA's 64 rows (the first row of the CTA and every row that starts a
-            // ray), with back-off: pairs that run out of coarse tiles early wait here for a whole tile time, and 148 x 512
-            // threads spinning on a handful of L2 lines starve the weight stream of the pairs still computing
+            // ray), with back-off: CTAs that run out of coarse tiles early wait here for a whole tile time, and
+            // hundreds of threads spinning on a handful of L2 lines starve the weight stream of the CTAs still computing
             if (gsub == 0 && (k == 0 || grow == 0) && pt_raw < P.total_points) {
               const volatile int* flag = p.rn.ready + ray;
               if (*flag == 0) {
@@ -570,15 +553,16 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1) k_field
           }
           for (int i = 0; i < 3; ++i) {
             d[i] = rr[3 + i];
-            x[i] = __fadd_rn(rr[i], __fmul_rn(zz, d[i]));  // nerf.py:185
+            xp[i] = __fadd_rn(rr[i], __fmul_rn(zz, d[i]));  // nerf.py:185
           }
         } else {
-          load_point(p.src, pt, x, d);
+          load_point(p.src, pt, xp, d);
         }
         for (int v = 0; v < NS; ++v) {
           // ---- geometry + the 42 input channels -> A chunk 0 (lin_in operand) ----
+          workers_sync();   // the previous view / tile is done with the geometry words and A chunk 0
           {
-            PointGeom pg = point_geometry(p.sc, sb, v, x, d);
+            PointGeom pg = point_geometry(p.sc, sb, v, xp, d);
             if (gsub == 0) {
               uint32_t* geo = reinterpret_cast<uint32_t*>(smem + SM_GEO) + grow * 8;
               const uint32_t vbase = (uint32_t)(sb * NS + v) * p.sc.Hl * p.sc.Wl;
@@ -594,8 +578,8 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1) k_field
             uint8_t* row_hi = smem + SM_A + grow * 128;
             uint8_t* row_lo = row_hi + 8192;
 #pragma unroll 1
-            for (int e = 0; e < 6; e += 2) {
-              const int ch = gsub * 6 + e;
+            for (int e = 0; e < 12; e += 2) {
+              const int ch = gsub * 12 + e;
               float f0 = feat_channel(pg, ch), f1 = feat_channel(pg, ch + 1);
               f0 = fmaxf(fminf(f0, 65504.f), -65504.f);
               f1 = fmaxf(fminf(f1, 65504.f), -65504.f);
@@ -603,65 +587,41 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1) k_field
               __half l0 = __float2half_rn(f0 - __half2float(h0)), l1 = __float2half_rn(f1 - __half2float(h1));
               const uint32_t hi = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
               const uint32_t lo = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-              const int byte = ((ch >> 3) ^ (grow & 7)) * 16 + (ch & 7) * 2;
-              *reinterpret_cast<uint32_t*>(row_hi + byte) = hi;
-              *reinterpret_cast<uint32_t*>(row_lo + byte) = lo;
+              const uint32_t byte = swz(grow, ch);
+              *reinterpret_cast<uint32_t*>(row_hi - grow * 128 + byte) = hi;
+              *reinterpret_cast<uint32_t*>(row_lo - grow * 128 + byte) = lo;
             }
             fence_proxy_async();
-            tc_fence_before();  // this warp's earlier TMEM reads (previous view / tile) precede the next lin_in MMA
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cta(bar_base + BAR_F_FULL * 8, 0);
-            workers_sync();  // geometry visible to all worker warps
+            workers_sync();  // geometry and the lin_in operand visible to both warpgroups
           }
-          // ---- lin_in, then blocks 0..2 ----
+          // ---- lin_in (overwrites X), then blocks 0..2 ----
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) x[q][i] = 0.f;   // X is dead until here: no registers held across the geometry
+          wide_steps<3>(rg, c, x, a0_desc, true);
+          epilogue_x<MODE_GATHER>(rg, c, x, nullptr, P.proj, nullptr, v, NS, nullptr, nullptr);
           for (int blk = 0; blk < 3; ++blk) {
-            const float* proj_blk = P.proj + (size_t)blk * map_stride;
-            if (blk == 0) {
-              for (int jj = 1; jj < 8; ++jj) stage_gather_chunk(smem, c.smem_u, proj_blk, chunk_order(jj), warp, lane);
-            }
-            epilogue<MODE_GATHER>(c, p, nullptr, X_COL, nullptr, proj_blk, v, nullptr, nullptr, acc_phase, blk != 0,
-                                  (fc_idx - 1) & 1, warp, 100 + 2 * blk);
-            acc_phase ^= 1;
-            ++fc_idx;
-            epilogue<MODE_HIDDEN>(c, p, nullptr, H_COL, P.fc0_b[blk], nullptr, v, nullptr, nullptr, acc_phase, true,
-                                  (fc_idx - 1) & 1, warp, 110 + 2 * blk);
-            acc_phase ^= 1;
-            ++fc_idx;
+            fc_block(rg, c, x, P.fc0_b[blk], p.status);
+            if (blk < 2)
+              epilogue_x<MODE_GATHER>(rg, c, x, nullptr, P.proj + (size_t)(blk + 1) * map_stride, nullptr, v, NS,
+                                      nullptr, nullptr);
+            else
+              epilogue_x<MODE_COMBINE>(rg, c, x, P.fc1_b[2], nullptr, nullptr, v, NS, scratch, nullptr);
           }
-          epilogue<MODE_COMBINE>(c, p, nullptr, X_COL, P.fc1_b[2], nullptr, v, scratch, nullptr, acc_phase, true,
-                                 (fc_idx - 1) & 1, warp, 120);
-          acc_phase ^= 1;
-          if (v == NS - 1) ++fc_idx;
         }
-        epilogue<MODE_HIDDEN>(c, p, nullptr, H_COL, P.fc0_b[3], nullptr, 0, nullptr, nullptr, acc_phase, true,
-                              (fc_idx - 1) & 1, warp, 130);
-        acc_phase ^= 1;
-        ++fc_idx;
-        epilogue<MODE_BIAS_WB>(c, p, nullptr, X_COL, P.fc1_b[3], nullptr, 0, nullptr, nullptr, acc_phase, true,
-                               (fc_idx - 1) & 1, warp, 132);
-        acc_phase ^= 1;
-        ++fc_idx;
-        epilogue<MODE_HIDDEN>(c, p, nullptr, H_COL, P.fc0_b[4], nullptr, 0, nullptr, nullptr, acc_phase, true,
-                              (fc_idx - 1) & 1, warp, 134);
-        acc_phase ^= 1;
-        ++fc_idx;
-        epilogue<MODE_OUT>(c, p, P.lin_out_w, X_COL, P.fc1_b[4], nullptr, 0, nullptr, out_part, acc_phase, false, 0,
-                           warp, 136);
-        acc_phase ^= 1;
-        tc_fence_before();
-        workers_sync();
+        fc_block(rg, c, x, P.fc0_b[3], p.status);
+        epilogue_x<MODE_BIAS_WB>(rg, c, x, P.fc1_b[3], nullptr, nullptr, 0, NS, nullptr, nullptr);
+        fc_block(rg, c, x, P.fc0_b[4], p.status);
+        epilogue_x<MODE_OUT>(rg, c, x, P.fc1_b[4], nullptr, P.lin_out_w, 0, NS, nullptr, out_part);
         if (threadIdx.x < ROWS) {
           const int64_t opt = tile * TILE_POINTS + rank * ROWS + threadIdx.x;
           if (opt < P.total_points) {
-            const float4* pp = reinterpret_cast<const float4*>(out_part) + threadIdx.x * 8;
-            float r0 = 0.f, r1 = 0.f, r2 = 0.f, r3 = 0.f;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const float4 a = pp[k];
-              r0 += a.x; r1 += a.y; r2 += a.z; r3 += a.w;
-            }
+            const float4 a = reinterpret_cast<const float4*>(out_part)[threadIdx.x * 2];
+            const float4 b = reinterpret_cast<const float4*>(out_part)[threadIdx.x * 2 + 1];
             const float* bo = P.lin_out_b;
-            r0 += bo[0]; r1 += bo[1]; r2 += bo[2]; r3 += bo[3];
+            const float r0 = (a.x + b.x) + bo[0], r1 = (a.y + b.y) + bo[1], r2 = (a.z + b.z) + bo[2],
+                        r3 = (a.w + b.w) + bo[3];
             float4 o;
             o.x = 1.0f / (1.0f + expf(-r0));   // sigmoid rgb, relu sigma (models.py:260-264)
             o.y = 1.0f / (1.0f + expf(-r1));
@@ -698,187 +658,41 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1) k_field
         const int n_done = *reinterpret_cast<volatile int*>(n_list);
         __threadfence();   // acquire side of the completion counters
         float* fs = reinterpret_cast<float*>(smem + SM_A + warp * FLUSH_SCRATCH_BYTES);
-        for (int i = warp; i < n_done; i += NWORKER_WARPS)
+        for (int i = warp; i < n_done; i += NCONSUMER_WARPS)
           finish_ray(p, ps, p.rn.lists[(size_t)blockIdx.x * p.rn.cap + i], fs, lane);
         workers_sync();
         if (threadIdx.x == 0) *n_list = 0;
         // (the next pass's first write to n_list happens after several workers_sync of its first tile)
       }
     }
-  } else if (warp == WARP_MMA) {
-    if (rank == 0) {
-      // =============================== MMA issuer (leader CTA) ===============================
-      // The whole warp runs this loop with warp-uniform values (descriptors live in uniform registers); only the
-      // tcgen05.mma / tcgen05.commit instructions themselves are predicated on one elected lane.
-      uint32_t seq = 0;          // weight-slot sequence number
-      uint32_t a_phase = 0, f_phase = 0;
-      long long t_afull = 0, t_alater = 0, t_bfull = 0, t_bpeer = 0;
-      const long long t_start = clock64();
-      const uint32_t a_base = smem_u32(smem + SM_A), b_base = smem_u32(smem + SM_B);
-      const uint64_t desc0 = make_desc(0);   // address field is added per operand (16-byte units)
-      const bool issuer = elect_one();
-      // one (feature block b, k-chunk j) step: W_hi slot (Ahi*Whi, Alo*Whi) then W_lo slot (Ahi*Wlo)
-      auto mma_step = [&](uint32_t d, int j, int ksteps, bool zero_acc, bool release_a) {
-        const uint64_t a_hi = desc0 + ((a_base + j * A_CHUNK_BYTES) >> 4);
-        const uint64_t a_lo = a_hi + (8192 >> 4);
-        {
-          const uint32_t sl = seq % NSLOTS, ph = (seq / NSLOTS) & 1;
-          mbar_wait_spin(bar_base + (BAR_B_FULL + sl) * 8, ph, p.status, 200 + sl, t_bfull);
-          mbar_wait_spin(bar_base + (BAR_B_PEER + sl) * 8, ph, p.status, 210 + sl, t_bpeer);
-          tc_fence_after();
-          const uint64_t bd = desc0 + ((b_base + sl * SLOT_BYTES) >> 4);
-          if (issuer) {
-            umma_f16_2sm(d, a_hi, bd, IDESC, zero_acc ? 0u : 1u);
-            umma_f16_2sm(d, a_hi + 2, bd + 2, IDESC, 1u);
-            umma_f16_2sm(d, a_hi + 4, bd + 4, IDESC, 1u);
-            if (ksteps == 4) umma_f16_2sm(d, a_hi + 6, bd + 6, IDESC, 1u);
-            umma_f16_2sm(d, a_lo, bd, IDESC, 1u);
-            umma_f16_2sm(d, a_lo + 2, bd + 2, IDESC, 1u);
-            umma_f16_2sm(d, a_lo + 4, bd + 4, IDESC, 1u);
-            if (ksteps == 4) umma_f16_2sm(d, a_lo + 6, bd + 6, IDESC, 1u);
-            umma_commit_pair(bar_base + (BAR_B_EMPTY + sl) * 8);
-          }
-          __syncwarp();
-          ++seq;
-        }
-        {
-          const uint32_t sl = seq % NSLOTS, ph = (seq / NSLOTS) & 1;
-          mbar_wait_spin(bar_base + (BAR_B_FULL + sl) * 8, ph, p.status, 200 + sl, t_bfull);
-          mbar_wait_spin(bar_base + (BAR_B_PEER + sl) * 8, ph, p.status, 210 + sl, t_bpeer);
-          tc_fence_after();
-          const uint64_t bd = desc0 + ((b_base + sl * SLOT_BYTES) >> 4);
-          if (issuer) {
-            umma_f16_2sm(d, a_hi, bd, IDESC, 1u);
-            umma_f16_2sm(d, a_hi + 2, bd + 2, IDESC, 1u);
-            umma_f16_2sm(d, a_hi + 4, bd + 4, IDESC, 1u);
-            if (ksteps == 4) umma_f16_2sm(d, a_hi + 6, bd + 6, IDESC, 1u);
-            umma_commit_pair(bar_base + (BAR_B_EMPTY + sl) * 8);
-            if (release_a) umma_commit_pair(bar_base + (BAR_A_FREE + j) * 8);
-          }
-          __syncwarp();
-          ++seq;
-        }
-      };
-      auto run_lin_in = [&]() {   // K = 42 -> 48, one chunk, both feature blocks
-#pragma unroll 1
-        for (int b = 0; b < 2; ++b) {
-          if (b == 0) mbar_wait_spin(bar_base + BAR_F_FULL * 8, f_phase, p.status, 220, t_afull);
-          mma_step(tmem_base + X_COL + b * 128, 0, 3, true, false);
-          if (issuer) umma_commit_pair(bar_base + (BAR_ACC + b) * 8);
-          __syncwarp();
-        }
-        f_phase ^= 1;
-      };
-      auto run_layer = [&](uint32_t dcol, bool overwrite) {
-        // Feature-block-major with a skew (fc_step_order): the epilogue of block 0 overlaps the tail of block 1 and
-        // the epilogue of block 1 overlaps the head of the next layer, both with about the same cover.  A chunks are
-        // waited for at their first use (block 0) and released after their last (block 1).
-#pragma unroll 1
-        for (int t = 0; t < 16; ++t) {
-          const int code = fc_step_order(t), b = code >> 3, jj = code & 7;
-          const int j = chunk_order(jj);
-          if (b == 0)
-            mbar_wait_spin(bar_base + (BAR_A_FULL + j) * 8, a_phase, p.status, 230 + j, jj == 0 ? t_afull : t_alater);
-          mma_step(tmem_base + dcol + b * 128, j, 4, overwrite && jj == 0, b == 1);
-          if (jj == 7) {
-            if (issuer) umma_commit_pair(bar_base + (BAR_ACC + b) * 8);
-            __syncwarp();
-          }
-        }
-        a_phase ^= 1;
-      };
-      for (int ps = 0; ps < p.npass; ++ps) {
-        const int64_t n_tiles = p.pass[ps].n_tiles;
-        for (int64_t tile = pair; tile < n_tiles; tile += n_pairs) {
-          for (int v = 0; v < NS; ++v) {
-            run_lin_in();
-            for (int blk = 0; blk < 3; ++blk) {
-              run_layer(H_COL, true);              // fc_0
-              run_layer(X_COL, false);             // fc_1 accumulates onto the residual
-            }
-          }
-          for (int blk = 3; blk < 5; ++blk) {
-            run_layer(H_COL, true);
-            run_layer(X_COL, false);
-          }
-        }
-      }
-      if (lane == 0) {
-        unsigned long long* cnt = reinterpret_cast<unsigned long long*>(p.status + 2);
-        atomicAdd(cnt + 0, (unsigned long long)(clock64() - t_start));
-        atomicAdd(cnt + 1, (unsigned long long)t_afull);
-        atomicAdd(cnt + 2, (unsigned long long)t_bfull);
-        atomicAdd(cnt + 3, (unsigned long long)t_bpeer);
-        atomicAdd(cnt + 6, (unsigned long long)t_alater);
-      }
-    } else if (lane == 0) {
-      // ============ peer CTA: forward "my half of the weight slot landed" to the leader ============
-      uint32_t seq = 0;
-      long long t_fwd = 0;
-      const uint32_t per_tile = (uint32_t)NS * (SLOTS_LIN_IN + 6 * SLOTS_FC) + 4 * SLOTS_FC;
-      for (int ps = 0; ps < p.npass; ++ps) {
-        const int64_t n_tiles = p.pass[ps].n_tiles;
-        for (int64_t tile = pair; tile < n_tiles; tile += n_pairs) {
-          for (uint32_t i = 0; i < per_tile; ++i) {
-            const uint32_t sl = seq % NSLOTS, ph = (seq / NSLOTS) & 1;
-            mbar_wait_spin(bar_base + (BAR_B_FULL + sl) * 8, ph, p.status, 300 + sl, t_fwd);
-            mbar_arrive_cta(bar_base + (BAR_B_PEER + sl) * 8, 0);
-            ++seq;
-          }
-        }
-      }
-    }
-  } else {
+  } else if (lane == 0) {
     // =============================== weight streamer ===============================
-    if (lane == 0) {
-      uint32_t seq = 0;
-      long long t_empty = 0;
-      const uint32_t b_base = smem_u32(smem + SM_B);
-      const uint8_t* slots = nullptr;
-      // (a bulk copy cannot complete on a barrier of another CTA than its destination -- tried, it faults -- so each
-      //  CTA streams its own half and the peer forwards "landed" to the leader)
-      auto stream_slot = [&](int slot_index) {
+    uint32_t seq = 0;
+    const uint32_t b_base = smem_u32(smem + SM_B);
+    const uint8_t* slots = nullptr;
+    auto stream = [&](int first, int count) {
+      for (int i = first; i < first + count; ++i) {
         const uint32_t sl = seq % NSLOTS, ph = (seq / NSLOTS) & 1;
-        mbar_wait_spin(bar_base + (BAR_B_EMPTY + sl) * 8, ph ^ 1, p.status, 400 + sl, t_empty);
-        const uint32_t full = bar_base + (BAR_B_FULL + sl) * 8;
+        mbar_wait(bar_base + (BAR_EMPTY + sl) * 8, ph ^ 1, p.status, 400 + sl);
+        const uint32_t full = bar_base + (BAR_FULL + sl) * 8;
         mbar_expect_tx(full, SLOT_BYTES);
-        bulk_g2s(b_base + sl * SLOT_BYTES, slots + (size_t)slot_index * SLOT_BYTES, SLOT_BYTES, full);
+        bulk_g2s(b_base + sl * SLOT_BYTES, slots + (size_t)i * SLOT_BYTES, SLOT_BYTES, full);
         ++seq;
-      };
-      auto stream_fc = [&](int layer) {  // layer 0..9 = fc_0/fc_1 of blocks 0..4, k-chunks in MMA order
-        const int base = SLOTS_LIN_IN + layer * SLOTS_FC;
-        for (int t = 0; t < 16; ++t) {
-          const int code = fc_step_order(t), b = code >> 3, jj = code & 7;
-          stream_slot(base + chunk_order(jj) * 4 + b * 2 + 0);
-          stream_slot(base + chunk_order(jj) * 4 + b * 2 + 1);
-        }
-      };
-      for (int ps = 0; ps < p.npass; ++ps) {
-        slots = p.pass[ps].packed + HEADER_BYTES + (size_t)rank * SLOTS_PER_RANK * SLOT_BYTES;
-        const int64_t n_tiles = p.pass[ps].n_tiles;
-        for (int64_t tile = pair; tile < n_tiles; tile += n_pairs) {
-          for (int v = 0; v < NS; ++v) {
-            for (int r = 0; r < SLOTS_LIN_IN; ++r) stream_slot(r);
-            for (int l = 0; l < 6; ++l) stream_fc(l);
-          }
-          for (int l = 6; l < 10; ++l) stream_fc(l);
-        }
       }
-      if (rank == 0) atomicAdd(reinterpret_cast<unsigned long long*>(p.status + 2) + 7, (unsigned long long)t_empty);
+    };
+    for (int ps = 0; ps < p.npass; ++ps) {
+      slots = p.pass[ps].packed + HEADER_BYTES;
+      const int64_t n_tiles = p.pass[ps].n_tiles;
+      for (int64_t tile = pair; tile < n_tiles; tile += n_pairs) {
+        for (int v = 0; v < NS; ++v) stream(0, SLOTS_LIN_IN + 3 * SLOTS_BLOCK);
+        stream(SLOTS_LIN_IN + 3 * SLOTS_BLOCK, 2 * SLOTS_BLOCK);
+      }
     }
-  }
-
-  // ---- teardown: everyone done with TMEM / peer smem before it is released ----
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == WARP_MMA) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
   }
 }
 
 // ---------------------------------------------------------------------------------------
-// weight packing: fp32 [512][K] -> fp16 hi/lo, per-rank 16 KB slots in MMA consumption order
+// weight packing: fp32 [512][K] -> fp16 hi/lo 16 KB slots (128 rows x 64 k, 128B-swizzled) in consumption order
 // ---------------------------------------------------------------------------------------
 __global__ void k_absmax(const float* __restrict__ w, int n, unsigned int* out) {
   float m = 0.f;
@@ -899,21 +713,45 @@ __global__ void k_pack_header(const unsigned int* absmax_bits, float* header) {
   header[1] = 1.0f / s;
 }
 
-// one block per slot: layer-local slot index ls = (j*2 + b)*2 + part
-__global__ void k_pack_layer(const float* __restrict__ W, int K, uint8_t* __restrict__ dst_rank0,
-                             uint8_t* __restrict__ dst_rank1, const float* __restrict__ header) {
-  const int ls = blockIdx.x, rank = blockIdx.y;
-  const int part = ls & 1, b = (ls >> 1) & 1, j = ls >> 2;
-  uint8_t* dst = (rank ? dst_rank1 : dst_rank0) + (size_t)ls * SLOT_BYTES;
-  const float s = header[0];
+// One block per slot.  lin_in (W1 == NULL, 8 slots): (N block q, part).
+// A ResNet block (128 slots): per hidden chunk hc, 16 fc_0 slots (k-chunk j, part) of W0 rows [128 hc, +128), then
+// 16 fc_1 slots (k-chunk jj of [128 hc, +128), N block q, part) of W1.
+__global__ void k_pack_slots(const float* __restrict__ W0, const float* __restrict__ W1, int K, uint8_t* __restrict__ dst,
+                             const float* __restrict__ header) {
+  const int s = blockIdx.x;
+  const float* W;
+  int part, n0, k0;
+  if (W1 == nullptr) {
+    const int q = s >> 1;
+    W = W0;
+    part = s & 1;
+    n0 = 128 * q;
+    k0 = 0;
+  } else {
+    const int hc = s >> 5, r = s & 31;
+    if (r < 16) {
+      W = W0;
+      part = r & 1;
+      n0 = 128 * hc;
+      k0 = 64 * (r >> 1);
+    } else {
+      const int r2 = r - 16, q = (r2 >> 1) & 3, jj = r2 >> 3;
+      W = W1;
+      part = r2 & 1;
+      n0 = 128 * q;
+      k0 = 64 * (2 * hc + jj);
+    }
+  }
+  uint8_t* out = dst + (size_t)s * SLOT_BYTES;
+  const float sc = header[0];
   for (int idx = threadIdx.x; idx < 128 * 64; idx += blockDim.x) {
     const int i = idx >> 6, kk = idx & 63;
-    const int n = b * 256 + rank * 128 + i, k = j * 64 + kk;
-    float w = (k < K) ? W[(size_t)n * K + k] * s : 0.f;
+    const int n = n0 + i, k = k0 + kk;
+    float w = (k < K) ? W[(size_t)n * K + k] * sc : 0.f;
     __half hi = __float2half_rn(w);
     __half val = part ? __float2half_rn(w - __half2float(hi)) : hi;
     const int byte = i * 128 + (((kk >> 3) ^ (i & 7)) * 16) + (kk & 7) * 2;
-    *reinterpret_cast<__half*>(dst + byte) = val;
+    *reinterpret_cast<__half*>(out + byte) = val;
   }
 }
 
@@ -958,7 +796,7 @@ bool tc_supported(const PnrScene& sc, const PnrMlp& m) {
 }
 
 static int tc_pairs(int64_t n_tiles) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   int64_t pairs = sms / 2;
@@ -966,7 +804,7 @@ static int tc_pairs(int64_t n_tiles) {
   return (int)(pairs < 1 ? 1 : pairs);
 }
 
-static size_t tc2_packed_bytes() { return (size_t)tc::HEADER_BYTES + (size_t)2 * tc::SLOTS_PER_RANK * tc::SLOT_BYTES; }
+static size_t tc_packed_bytes() { return (size_t)tc::HEADER_BYTES + (size_t)tc::SLOTS_TOTAL * tc::SLOT_BYTES; }
 
 size_t tc_workspace_bytes(const PnrScene&, const PnrMlp&, int64_t total_points) {
   int64_t n_tiles = (total_points + tc::TILE_POINTS - 1) / tc::TILE_POINTS;
@@ -1126,7 +964,7 @@ extern "C" {
 
 size_t pnr_pack_mlp_bytes(const PnrMlp* mlp) {
   if (!mlp || mlp->d_hidden != tc::D || mlp->d_latent != tc::D || mlp->n_blocks != 5 || mlp->d_in != 42) return 0;
-  return tc2_packed_bytes();
+  return tc_packed_bytes();
 }
 
 int pnr_pack_mlp(const PnrMlp* mlp, void* packed, size_t packed_bytes, void* stream) {
@@ -1153,16 +991,12 @@ int pnr_pack_mlp(const PnrMlp* mlp, void* packed, size_t packed_bytes, void* str
   }
   tc::k_pack_header<<<1, 1, 0, s>>>(absmax, header);
   PNR_LAUNCH_CHECK();
-  uint8_t* r0 = base + tc::HEADER_BYTES;
-  uint8_t* r1 = r0 + (size_t)tc::SLOTS_PER_RANK * tc::SLOT_BYTES;
-  tc::k_pack_layer<<<dim3(tc::SLOTS_LIN_IN, 2), 256, 0, s>>>(mlp->lin_in_w, mlp->d_in, r0, r1, header);
+  uint8_t* slots = base + tc::HEADER_BYTES;
+  tc::k_pack_slots<<<tc::SLOTS_LIN_IN, 256, 0, s>>>(mlp->lin_in_w, nullptr, mlp->d_in, slots, header);
   PNR_LAUNCH_CHECK();
   for (int i = 0; i < 5; ++i) {
-    size_t o0 = (size_t)(tc::SLOTS_LIN_IN + (2 * i) * tc::SLOTS_FC) * tc::SLOT_BYTES;
-    size_t o1 = (size_t)(tc::SLOTS_LIN_IN + (2 * i + 1) * tc::SLOTS_FC) * tc::SLOT_BYTES;
-    tc::k_pack_layer<<<dim3(tc::SLOTS_FC, 2), 256, 0, s>>>(mlp->fc0_w[i], tc::D, r0 + o0, r1 + o0, header);
-    PNR_LAUNCH_CHECK();
-    tc::k_pack_layer<<<dim3(tc::SLOTS_FC, 2), 256, 0, s>>>(mlp->fc1_w[i], tc::D, r0 + o1, r1 + o1, header);
+    uint8_t* dst = slots + (size_t)(tc::SLOTS_LIN_IN + i * tc::SLOTS_BLOCK) * tc::SLOT_BYTES;
+    tc::k_pack_slots<<<tc::SLOTS_BLOCK, 256, 0, s>>>(mlp->fc0_w[i], mlp->fc1_w[i], tc::D, dst, header);
     PNR_LAUNCH_CHECK();
   }
   return PNR_OK;
@@ -1191,7 +1025,7 @@ int pnr_project_latent(const PnrScene* sc, const PnrMlp* mlp, float* proj, size_
     const float* extra = (i == 0) ? mlp->lin_in_b : mlp->fc1_b[i - 1];
     tc::k_proj_bias<<<2, 256, 0, s>>>(mlp->lin_z_b[i], extra, bias + i * tc::D, tc::D);
     PNR_LAUNCH_CHECK();
-    // fp16 hi/lo split tcgen05 GEMM (22 mantissa bits, the precision of the fused kernel's own products);
+    // fp16 hi/lo split tensor-core GEMM (22 mantissa bits, the precision of the fused kernel's own products);
     // PNR_PROJECT_SIMT=1 keeps the fp32 FFMA SGEMM of round 1
     static const bool simt = getenv("PNR_PROJECT_SIMT") != nullptr;
     int rc = simt ? sgemm(sc->latent_nhwc, tc::D, mlp->lin_z_w[i], bias + i * tc::D, proj + (size_t)i * rows * tc::D,
@@ -1219,11 +1053,8 @@ int pnr_tc_status(int* out) {
 }
 
 
-// Debug: cycle breakdown accumulated over all launches since the last call (summed over the leader CTAs):
-// [0] MMA warp total, [1] its waits for the FIRST A chunk of a layer (layer-boundary bubble), [2] for its own weight
-// slot, [3] for the peer's slot, [4], [5] unused (0),
-// [6] MMA waits for later A chunks, [7] streamer waits for a free slot.
-// (M-split variant; the N-split variant fills [0] total, [1] chunk waits, [2] weight waits, [4..6] worker totals.)
+// Debug: 8 cycle counters accumulated over all launches since the last call; clears them.  The wgmma kernel
+// records none, so they read 0.
 int pnr_tc_counters(unsigned long long* out8) {
   int* buf = nullptr;
   int rc = tc::get_status_buffer(&buf);

@@ -3,19 +3,20 @@
 // i.e. the signature of the SIMT `sgemm` (pnr_field_simt.cu) it replaces inside field_backward: the recomputed forward
 // layers, dX = dY W (on W^T) and dW += dY^T X (on transposed panels, K = rows, split-K).
 //
-// tcgen05 (cta_group::1, UMMA M128 N128 K16, kind::f16 with BF16 operands), accumulator in TMEM.  Each fp32 operand
+// wgmma (sm_90a warpgroup MMA, m64n128k16 with BF16 operands), accumulators in registers.  Each fp32 operand
 // is split on the fly into an error-compensated bf16 pair x = hi + lo (16 mantissa bits; bf16 keeps fp32's exponent
 // range, so the tiny values of a backward pass need no scaling) and D += Ahi*Bhi + Alo*Bhi + Ahi*Blo: 3 tensor
 // passes per GEMM, measured worst relative gradient error 1.4e-5 (scripts/precision_study_backward.py), two orders
 // below the 1e-3 the gradient tests allow.
 //
-// CTA = 8 producer/epilogue warps + 1 MMA warp, one 128x128 output tile over a K range:
-//   producers : coalesced LDG.128 of the fp32 operands -> (ReLU) -> bf16 hi/lo -> st.shared into K-major
-//               128B-swizzled tiles (the layout pnr_field_tc.cu uses), 3-stage ring, mbarrier full/empty
-//   MMA warp  : one elected lane issues 12 MMAs per 64-wide k-step, tcgen05.commit frees the stage
-//   epilogue  : tcgen05.ld -> (+ bias) -> store / read-add-store / red.global.add (split-K)
+// CTA = 2 warpgroups, one 128x128 output tile over a K range; every thread loads, splits and consumes:
+//   load     : coalesced LDG.128 of the fp32 operands -> (ReLU) -> bf16 hi/lo -> st.shared into K-major
+//              128B-swizzled tiles (the layout pnr_field_tc.cu uses), 3-stage ring
+//   MMA      : each warpgroup issues 12 wgmma per 64-wide k-step for its 64 rows and keeps one k-step in flight
+//              while the next one is loaded
+//   epilogue : registers -> (+ bias) -> store / read-add-store / red.global.add (split-K)
 // Roofline: tensor-bound for large K, but both operands arrive as fp32 through L2 (8 B per bf16-pair element), so
-// the practical bound is L2->SM bandwidth: 64 KB of operands per 6.3 M MAC k-step.
+// the practical bound is L2->SM bandwidth: 64 KB of operands per 1 M MAC k-step.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -25,8 +26,6 @@
 
 namespace pnr {
 
-int tc_status_buffer(int** out);   // pnr_field_tc.cu
-
 namespace gemmtc {
 
 using namespace tcptx;
@@ -35,13 +34,8 @@ constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int STAGES = 3;
 constexpr int TILE_BYTES = 128 * 128;          // 128 rows x 64 bf16
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;    // A hi, A lo, B hi, B lo
-constexpr int NPROD_WARPS = 8;
-constexpr int NTHREADS = (NPROD_WARPS + 1) * 32;
-constexpr int SM_BAR = STAGES * STAGE_BYTES;
-constexpr int SMEM_BYTES = SM_BAR + 256;
-// kind::f16: D = F32 (bit 4), A / B format BF16 (bits 7, 10 set) or F16 (clear), both K-major, N = 128, M = 128
-constexpr uint32_t IDESC_F16 = (1u << 4) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-constexpr uint32_t IDESC_BF16 = IDESC_F16 | (1u << 7) | (1u << 10);
+constexpr int NTHREADS = 256;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES;
 
 struct Params {
   const float* A;
@@ -52,7 +46,6 @@ struct Params {
   int k_per_split;   // multiple of BK
   int relu_a, mode;  // mode 0: store, 1: C += (single split), 2: atomic add (split-K)
   const float* mask; // optional [M][ldc]: the product is zeroed where mask <= 0 (ReLU backward) before store / add
-  int* status;
 };
 
 // 8 fp32 values -> error-compensated 16-bit pairs x = hi + lo.  BF16: 8 + 8 mantissa bits with fp32's exponent range
@@ -86,164 +79,102 @@ __device__ __forceinline__ void split8(const float4 a, const float4 b, bool relu
 
 template <bool BF16>
 __global__ void __launch_bounds__(NTHREADS, 1) k_gemm_split3(const __grid_constant__ Params p) {
-  constexpr uint32_t IDESC = BF16 ? IDESC_BF16 : IDESC_F16;
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t = threadIdx.x, wg = t >> 7, warp = t >> 5, lane = t & 31;
   const uint32_t smem_u = smem_u32(smem);
-  const uint32_t bar = smem_u + SM_BAR;               // full[STAGES], empty[STAGES], acc
-  const uint32_t bar_full = bar, bar_empty = bar + STAGES * 8, bar_acc = bar + 2 * STAGES * 8;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BAR + 128);
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
   const int k_begin = blockIdx.z * p.k_per_split;
   const int k_end = min(p.K, k_begin + p.k_per_split);
   const int nk = (k_end - k_begin + BK - 1) / BK;
   if (nk <= 0) return;   // (cannot happen with the host's split computation; uniform over the CTA)
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(bar_full + i * 8, NPROD_WARPS);
-      mbar_init(bar_empty + i * 8, 1);
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  const uint64_t desc0 = make_desc(0);
+  for (int it = 0; it < nk; ++it) {
+    const int st = it % STAGES;
+    const int k0 = k_begin + it * BK;
+    // all 16 loads in flight before the first use
+    float4 va[4][2], vb[4][2];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int id = t + 256 * i, row = id >> 3, u = id & 7;
+      const int k = k0 + u * 8;
+      const bool ka = k < k_end;
+      const int m = m0 + row, n = n0 + row;
+      if (ka && m < p.M) {
+        const float4* src = reinterpret_cast<const float4*>(p.A + (size_t)m * p.lda + k);
+        va[i][0] = __ldg(src);
+        va[i][1] = __ldg(src + 1);
+      } else {
+        va[i][0] = va[i][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      if (ka && n < p.N) {
+        const float4* src = reinterpret_cast<const float4*>(p.W + (size_t)n * p.ldw + k);
+        vb[i][0] = __ldg(src);
+        vb[i][1] = __ldg(src + 1);
+      } else {
+        vb[i][0] = vb[i][1] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
     }
-    mbar_init(bar_acc, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    // stage `st` was last read by the wgmma of step it - STAGES, which both warpgroups waited for (wait_group 1 at
+    // the end of step it - STAGES + 1) before the barrier of step it - 1
+    const uint32_t sbase = smem_u + st * STAGE_BYTES;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int id = t + 256 * i, row = id >> 3, u = id & 7;
+      const uint32_t off = (uint32_t)(row * 128 + ((u ^ (row & 7)) * 16));
+      uint4 hi, lo;
+      split8<BF16>(va[i][0], va[i][1], p.relu_a != 0, hi, lo);
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + off), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w) : "memory");
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + TILE_BYTES + off), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
+      split8<BF16>(vb[i][0], vb[i][1], false, hi, lo);
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + 2 * TILE_BYTES + off), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w) : "memory");
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + 3 * TILE_BYTES + off), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
+    }
+    fence_proxy_async();
+    __syncthreads();
+    // warpgroup wg: rows [64 wg, 64 wg + 64) of the A tile against all 128 rows of the B tile
+    const uint64_t a_hi = desc0 + ((sbase + wg * (TILE_BYTES / 2)) >> 4), a_lo = a_hi + (TILE_BYTES >> 4);
+    const uint64_t b_hi = desc0 + ((sbase + 2 * TILE_BYTES) >> 4), b_lo = b_hi + (TILE_BYTES >> 4);
+    fence_acc<64>(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      if (BF16) {
+        wgmma_m64n128_bf16(acc, a_hi + 2 * kk, b_hi + 2 * kk, (it | kk) ? 1u : 0u);
+        wgmma_m64n128_bf16(acc, a_lo + 2 * kk, b_hi + 2 * kk, 1u);
+        wgmma_m64n128_bf16(acc, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
+      } else {
+        wgmma_m64n128_f16(acc, a_hi + 2 * kk, b_hi + 2 * kk, (it | kk) ? 1u : 0u);
+        wgmma_m64n128_f16(acc, a_lo + 2 * kk, b_hi + 2 * kk, 1u);
+        wgmma_m64n128_f16(acc, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    fence_acc<64>(acc);
   }
-  if (warp == NPROD_WARPS) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(128u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  wgmma_wait<0>();
+  fence_acc<64>(acc);
 
-  if (warp < NPROD_WARPS) {
-    // ------------------------------ producers ------------------------------
-    const int t = threadIdx.x;          // 0..255
-    for (int it = 0; it < nk; ++it) {
-      const int st = it % STAGES;
-      const uint32_t ph = (it / STAGES) & 1;
-      const int k0 = k_begin + it * BK;
-      // all 16 loads in flight before the first use
-      float4 va[4][2], vb[4][2];
+  // ------------------------------ epilogue ------------------------------
+  const bool add_bias = p.bias != nullptr && blockIdx.z == 0;
+  const int rbase = m0 + wg * 64 + 16 * (warp & 3) + (lane >> 2);
+  const int cbase = n0 + 2 * (lane & 3);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int id = t + 256 * i, row = id >> 3, u = id & 7;
-        const int k = k0 + u * 8;
-        const bool ka = k < k_end;
-        const int m = m0 + row, n = n0 + row;
-        if (ka && m < p.M) {
-          const float4* src = reinterpret_cast<const float4*>(p.A + (size_t)m * p.lda + k);
-          va[i][0] = __ldg(src);
-          va[i][1] = __ldg(src + 1);
-        } else {
-          va[i][0] = va[i][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-        if (ka && n < p.N) {
-          const float4* src = reinterpret_cast<const float4*>(p.W + (size_t)n * p.ldw + k);
-          vb[i][0] = __ldg(src);
-          vb[i][1] = __ldg(src + 1);
-        } else {
-          vb[i][0] = vb[i][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-      mbar_wait(bar_empty + st * 8, ph ^ 1, p.status, 500 + st);
-      const uint32_t sbase = smem_u + st * STAGE_BYTES;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int id = t + 256 * i, row = id >> 3, u = id & 7;
-        const uint32_t off = (uint32_t)(row * 128 + ((u ^ (row & 7)) * 16));
-        uint4 hi, lo;
-        split8<BF16>(va[i][0], va[i][1], p.relu_a != 0, hi, lo);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + off), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + TILE_BYTES + off), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
-        split8<BF16>(vb[i][0], vb[i][1], false, hi, lo);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + 2 * TILE_BYTES + off), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + 3 * TILE_BYTES + off), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_full + st * 8);
-    }
-    // ------------------------------ epilogue ------------------------------
-    mbar_wait(bar_acc, 0, p.status, 510);
-    tc_fence_after();
-    const int q = warp & 3, half = warp >> 2;
-    const int row = 32 * q + lane;
-    const int m = m0 + row;
-    const uint32_t taddr = tmem + ((uint32_t)(32 * q) << 16) + (uint32_t)(half * 64);
-#pragma unroll 1
-    for (int c16 = 0; c16 < 4; ++c16) {
-      float v[16];
-      tmem_ld16(taddr + c16 * 16, v);
-      const int nb = n0 + half * 64 + c16 * 16;
-      if (m < p.M) {
-        float* dst = p.C + (size_t)m * p.ldc + nb;
-        const bool add_bias = p.bias != nullptr && blockIdx.z == 0;
-        if (p.mask) {
-          const float* mk = p.mask + (size_t)m * p.ldc + nb;
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (nb + j < p.N && !(mk[j] > 0.f)) v[j] = 0.f;
-        }
-        if (nb + 16 <= p.N && p.mode != 2 && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            float4 o = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
-            if (add_bias) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + nb) + j4);
-              o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w;
-            }
-            float4* d4 = reinterpret_cast<float4*>(dst) + j4;
-            if (p.mode == 1) {
-              const float4 c = *d4;
-              o.x += c.x; o.y += c.y; o.z += c.z; o.w += c.w;
-            }
-            *d4 = o;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (nb + j >= p.N) continue;
-            float o = v[j] + (add_bias ? p.bias[nb + j] : 0.f);
-            if (p.mode == 2) atomicAdd(dst + j, o);
-            else if (p.mode == 1) dst[j] += o;
-            else dst[j] = o;
-          }
-        }
-      }
-    }
-    tc_fence_before();
-  } else {
-    // ------------------------------ MMA issuer ------------------------------
-    const bool issuer = elect_one();
-    long long t_wait = 0;
-    const uint64_t desc0 = make_desc(0);
-    for (int it = 0; it < nk; ++it) {
-      const int st = it % STAGES;
-      const uint32_t ph = (it / STAGES) & 1;
-      mbar_wait_spin(bar_full + st * 8, ph, p.status, 520 + st, t_wait);
-      tc_fence_after();
-      const uint32_t sbase = smem_u + st * STAGE_BYTES;
-      const uint64_t a_hi = desc0 + (sbase >> 4), a_lo = a_hi + (TILE_BYTES >> 4);
-      const uint64_t b_hi = a_hi + (2 * TILE_BYTES >> 4), b_lo = a_hi + (3 * TILE_BYTES >> 4);
-      if (issuer) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          umma_f16_1sm(tmem, a_hi + 2 * kk, b_hi + 2 * kk, IDESC, (it | kk) ? 1u : 0u);
-          umma_f16_1sm(tmem, a_lo + 2 * kk, b_hi + 2 * kk, IDESC, 1u);
-          umma_f16_1sm(tmem, a_hi + 2 * kk, b_lo + 2 * kk, IDESC, 1u);
-        }
-        umma_commit_local(bar_empty + st * 8);
-        if (it == nk - 1) umma_commit_local(bar_acc);
-      }
-      __syncwarp();
-    }
-  }
-  __syncthreads();
-  tc_fence_after();
-  if (warp == NPROD_WARPS) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128u) : "memory");
+  for (int i = 0; i < 64; ++i) {
+    const int m = rbase + 8 * ((i >> 1) & 1);
+    const int n = cbase + 8 * (i >> 2) + (i & 1);
+    if (m >= p.M || n >= p.N) continue;
+    float o = acc[i];
+    if (p.mask && !(p.mask[(size_t)m * p.ldc + n] > 0.f)) o = 0.f;
+    if (add_bias) o += __ldg(p.bias + n);
+    float* dst = p.C + (size_t)m * p.ldc + n;
+    if (p.mode == 2) atomicAdd(dst, o);
+    else if (p.mode == 1) *dst += o;
+    else *dst = o;
   }
 }
 
@@ -266,14 +197,15 @@ static int gemm_split3(bool bf16, const float* A, int lda, const float* W, int l
     set_error("tensor-core gemm: mask and bias together are not supported");
     return PNR_ERR_INVALID;
   }
-  int rc = tc_status_buffer(&p.status);
-  if (rc) return rc;
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
   const int ksteps = (K + BK - 1) / BK;
   // split K when the output has too few tiles to fill the GPU (the weight-gradient GEMMs: 512 x 512 over K = rows)
   int splits = 1;
-  if (tiles < 148 && ksteps >= 8) {
-    splits = (2 * 148 + tiles - 1) / tiles;
+  if (tiles < sms && ksteps >= 8) {
+    splits = (2 * sms + tiles - 1) / tiles;
     if (splits > ksteps / 4) splits = ksteps / 4;
     if (splits < 1) splits = 1;
   }
@@ -283,8 +215,6 @@ static int gemm_split3(bool bf16, const float* A, int lda, const float* W, int l
   p.mode = splits > 1 ? 2 : (accum ? 1 : 0);
   if (splits > 1 && !accum) PNR_CUDA(cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, s));
   static bool attr_set[64] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
     PNR_CUDA(cudaFuncSetAttribute(k_gemm_split3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     PNR_CUDA(cudaFuncSetAttribute(k_gemm_split3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));

@@ -1,4 +1,4 @@
-// PTX wrappers (mbarrier, bulk copy, tcgen05, fences) shared by the tensor-engine kernels.
+// PTX wrappers (mbarrier, bulk copy, wgmma, fences) shared by the tensor-engine kernels (sm_90a).
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -15,7 +15,7 @@ __device__ __forceinline__ long long timeout_limit(const int* status) {
 }
 
 // ---------------------------------------------------------------------------------------
-// PTX wrappers
+// mbarrier / bulk copy
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -24,11 +24,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cta(uint32_t bar, uint32_t cta) {  // barrier of CTA `cta` of the pair
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(bar), "r"(cta));
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(r) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -44,9 +39,6 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity)
       : "memory");
   return ok;
 }
-// Waits use CTA-scope try_wait (what CUTLASS's ClusterBarrier does): a cluster-scope acquire would make ptxas
-// emit CCTL.IVALL (an L1 invalidate) on every spin.  The data these barriers guard is read by the async proxy
-// (tensor core / TMA), which the producers order with fence.proxy.async before arriving.
 static __device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity, int* status, int tag) {
   long long t0 = clock64();
   uint32_t spins = 0;
@@ -61,44 +53,9 @@ static __device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity
     }
   }
 }
-// Latency-critical single waiters (MMA issuer, weight streamer, forwarder) spin without the suspend hint: a parked
-// warp wakes up noticeably later than a spinning one, and these few threads cost no meaningful issue bandwidth.
-__device__ __forceinline__ uint32_t mbar_try_wait_nohint(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok;
-}
-__device__ __forceinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity, int* status, int tag, long long& acc) {
-  const long long t0 = clock64();
-  uint32_t spins = 0;
-  while (!mbar_try_wait_nohint(bar, parity)) {
-    if ((++spins & 0xFFF) == 0) {
-      if (*(volatile int*)status != 0) break;
-      if (clock64() - t0 > timeout_limit(status)) {
-        atomicCAS(status, 0, tag);
-        if (((volatile int*)status)[1]) __trap();
-        break;
-      }
-    }
-  }
-  acc += clock64() - t0;
-}
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* status, int tag) {
   if (mbar_try_wait(bar, parity)) return;
   mbar_wait_slow(bar, parity, status, tag);
-}
-
-// wait and add the stalled cycles to a per-thread counter (debug breakdown, see pnr_tc_counters)
-__device__ __forceinline__ void mbar_wait_timed(uint32_t bar, uint32_t parity, int* status, int tag, long long& acc) {
-  const long long t0 = clock64();   // the first try_wait may already sleep (suspend-time hint), so time it too
-  if (!mbar_try_wait(bar, parity)) mbar_wait_slow(bar, parity, status, tag);
-  acc += clock64() - t0;
 }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
@@ -106,223 +63,68 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// generic-proxy shared-memory writes (operand tiles) become visible to the async proxy (wgmma)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void workers_sync() { asm volatile("bar.sync 1, 512;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; one thread issues for the CTA pair.
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// ---------------------------------------------------------------------------------------
+// wgmma (warpgroup MMA): D[64 x N] (+)= A[smem desc] * B[smem desc]^T, fp32 accumulators in registers.
+// Accumulator element i of thread t (warp w = t/32 of the warpgroup, lane l):
+//   row = 16 w + l/4 + 8 ((i >> 1) & 1),   col = 8 (i >> 2) + 2 (l % 4) + (i & 1)
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// all previously issued MMAs complete -> arrive on the barrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"((uint16_t)3)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accumulator reads / writes across a wgmma issue or wait
+template <int N>
+__device__ __forceinline__ void fence_acc(float* d) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-               "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-               "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-               "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-               : "memory");
-}
-// k-chunks of a layer are produced by the workers in 4 waves (0,2 | 1,3 | 4,6 | 5,7); the MMA consumes in that order
-__device__ __forceinline__ int chunk_order(int jj) { return (jj & 4) | ((jj & 1) << 1) | ((jj >> 1) & 1); }
-// Order of the 16 (feature block b, chunk position jj) steps of a 512x512 layer, as b*8+jj.  Block 0 over chunk
-// positions 0-3, PNR_TC_SKEW early block-1 steps, block 0 over 4-7, the rest of block 1.  Skew 0 is plain block-major.
-#ifndef PNR_TC_SKEW
-#define PNR_TC_SKEW 0
-#endif
-__device__ __forceinline__ int fc_step_order(int t) {
-  if (t < 4) return t;                                   // b0 jj 0..3
-  if (t < 4 + PNR_TC_SKEW) return 8 + (t - 4);           // b1 jj 0..SKEW-1
-  if (t < 8 + PNR_TC_SKEW) return t - PNR_TC_SKEW;       // b0 jj 4..7
-  return t;                                              // b1 jj SKEW..7
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// K-major, 128B-swizzled operand tile: rows of 128 B, 8-row groups 1024 B apart.
+// K-major, 128B-swizzled operand tile: rows of 128 B (64 16-bit values), 8-row groups 1024 B apart.  The tile base
+// must be 1024-byte aligned; the k16 step inside a row is +32 B (+2 in the address field).
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;             // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;   // stride byte offset
-  d |= (uint64_t)1 << 46;             // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;             // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;             // SWIZZLE_128B
   return d;
 }
-// kind::f16, A/B = F16 K-major, D = F32, M = 128 (64 rows per CTA), N = 256
-constexpr uint32_t IDESC_M128_N256 = (1u << 4) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
 
-__device__ __forceinline__ uint32_t split_pack(float a0, float a1, uint32_t& lo_out) {
-  a0 = fminf(a0, 65504.f);
-  a1 = fminf(a1, 65504.f);
-  __half h0 = __float2half_rn(a0), h1 = __float2half_rn(a1);
-  __half l0 = __float2half_rn(a0 - __half2float(h0)), l1 = __float2half_rn(a1 - __half2float(h1));
-  lo_out = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-  return (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-}
-
-// relu(y[0..15]) -> fp16 hi/lo -> swizzled A tile (row m, k columns [16g, 16g+16) of chunk at `chunk`)
-__device__ __forceinline__ void store_a16(uint8_t* chunk, int m, int g, const float* y) {
-  uint32_t hi[8], lo[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) hi[e] = split_pack(fmaxf(y[2 * e], 0.f), fmaxf(y[2 * e + 1], 0.f), lo[e]);
-  uint8_t* row_hi = chunk + m * 128;
-  uint8_t* row_lo = row_hi + 8192;
-  const int u0 = (2 * g) ^ (m & 7), u1 = (2 * g + 1) ^ (m & 7);
-  *reinterpret_cast<uint4*>(row_hi + u0 * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-  *reinterpret_cast<uint4*>(row_hi + u1 * 16) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-  *reinterpret_cast<uint4*>(row_lo + u0 * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-  *reinterpret_cast<uint4*>(row_lo + u1 * 16) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-}
-
-
-}  // namespace tcptx
-}  // namespace pnr
-
-// ---- additions for the N-split (cta_group::1 + DSMEM) kernel --------------------------------------
-namespace pnr {
-namespace tcptx {
-
-__device__ __forceinline__ uint32_t mapa_cluster(uint32_t saddr, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(cta));
-  return r;
-}
-__device__ __forceinline__ void st_cluster_v4(uint32_t raddr, uint4 v) {
-  asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(raddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
-               : "memory");
-}
-// asynchronous DSMEM store: 16 bytes to the peer's shared memory, completing 16 tx-bytes on the peer's mbarrier
-__device__ __forceinline__ void st_async_v4(uint32_t raddr, uint4 v, uint32_t rbar) {
-  asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];" ::"r"(raddr),
-               "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(rbar)
-               : "memory");
-}
-__device__ __forceinline__ void st_cluster_f32(uint32_t raddr, float v) {
-  asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(raddr), "f"(v) : "memory");
-}
-// arrive on a barrier of CTA `cta` with cluster-scope release (orders this thread's prior DSMEM stores)
-__device__ __forceinline__ void mbar_arrive_cta_release(uint32_t bar, uint32_t cta) {
-  uint32_t r = mapa_cluster(bar, cta);
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(r) : "memory");
-}
-__device__ __forceinline__ uint32_t mbar_try_wait_cluster(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
+__device__ __forceinline__ void wgmma_m64n64_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity), "r"(0x989680u)
-      : "memory");
-  return ok;
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-static __device__ __noinline__ void mbar_wait_cluster_slow(uint32_t bar, uint32_t parity, int* status, int tag) {
-  long long t0 = clock64();
-  uint32_t spins = 0;
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if ((++spins & 0x3F) == 0) {
-      if (*(volatile int*)status != 0) return;
-      if (clock64() - t0 > timeout_limit(status)) {
-        atomicCAS(status, 0, tag);
-        if (((volatile int*)status)[1]) __trap();   // default: fail the launch loudly (see get_status_buffer)
-        return;
-      }
-    }
-  }
-}
-// wait that also acquires at cluster scope: for data written into this CTA's smem by the peer's threads
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity, int* status, int tag, long long& acc) {
-  if (mbar_try_wait_cluster(bar, parity)) return;
-  const long long t0 = clock64();
-  mbar_wait_cluster_slow(bar, parity, status, tag);
-  acc += clock64() - t0;
-}
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_f16_1sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n128_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit_local(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// arrive on the barrier at this offset in BOTH CTAs of the pair once all prior MMAs of this CTA are done
-__device__ __forceinline__ void umma_commit_both(uint32_t bar) {
+__device__ __forceinline__ void wgmma_m64n128_bf16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"((uint16_t)3)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float* v) {
-  uint32_t r[4];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 4; ++i) v[i] = __uint_as_float(r[i]);
-}
-constexpr uint32_t IDESC_M128_N16 = (1u << 4) | ((16u >> 3) << 17) | ((128u >> 4) << 24);
 
 }  // namespace tcptx
 }  // namespace pnr

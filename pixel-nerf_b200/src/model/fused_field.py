@@ -2,7 +2,7 @@
 
 Used whenever `net(xyz, ...)` itself is called with gradients required (a whole training step through
 `NeRFRenderer` uses the render-level node of render/fused_train.py instead; `PNR_FUSED_BACKWARD=1` forces this
-field-level node there too, `=0` the composed-torch path).  Validated on B200 (tests/test_gpu_backward.py).
+field-level node there too, `=0` the composed-torch path).  Validated on H100 (tests/test_gpu_backward.py).
 
 The autograd node takes the sample positions, the latent and the MLP parameters as inputs, so autograd carries
 `d_xyz` back into the renderer (sample depths), `d_latent` into the encoder trunk and the weight gradients into the

@@ -2,7 +2,7 @@
 PixelNeRFNet with the reference's surface (src/model/models.py): `encode()` leaves the scene
 state in module buffers, `forward(xyz, coarse, viewdirs)` evaluates the conditioned field.
 
-Inference (no autograd) goes to the fused sm_100a kernels through the C ABI
+Inference (no autograd) goes to the fused sm_90a kernels through the C ABI
 (`pnr_field_eval`, include/pnr.h); there is no CPU fallback on that path.  When gradients are
 required on CUDA (train/train.py) the same fused forward runs inside an autograd node whose
 backward is `pnr_field_backward` (model/fused_field.py; SURVEY.md section 8f row 1).  The

@@ -1,5 +1,5 @@
 """
-ctypes binding of libpnr_sm100.so (C ABI: include/pnr.h) -- the only way the Python host
+ctypes binding of libpnr_sm90.so (C ABI: include/pnr.h) -- the only way the Python host
 code reaches the GPU kernels.  There is no fallback: if the library is missing, or a tensor
 is not a contiguous fp32 CUDA tensor, the call raises.
 
@@ -11,7 +11,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.realpath(__file__))   # realpath: `src/` may be reached through an overlay symlink
-LIB_PATH = os.environ.get("PNR_LIB", os.path.join(os.path.dirname(_HERE), "lib", "libpnr_sm100.so"))
+LIB_PATH = os.environ.get("PNR_LIB", os.path.join(os.path.dirname(_HERE), "lib", "libpnr_sm90.so"))
 
 PNR_MAX_BLOCKS = 8
 ENGINE_AUTO, ENGINE_SIMT, ENGINE_TC = 0, 1, 2
@@ -130,18 +130,18 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"libpnr_sm100.so not found at {LIB_PATH}: build it with `python -c 'import __graft_entry__ as g; "
+            f"libpnr_sm90.so not found at {LIB_PATH}: build it with `python -c 'import __graft_entry__ as g; "
             "g.build()'` (or `make -C pixel-nerf_b200/csrc`). There is no CPU fallback for the render path.")
     L = declare(C.CDLL(LIB_PATH))
     if L.pnr_abi_version() != 2:
-        raise RuntimeError("libpnr_sm100.so ABI version mismatch")
+        raise RuntimeError("libpnr_sm90.so ABI version mismatch")
     _lib = L
     return L
 
 
 def check(rc):
     if rc != 0:
-        raise RuntimeError(f"libpnr_sm100 error {rc}: {lib().pnr_last_error().decode()}")
+        raise RuntimeError(f"libpnr_sm90 error {rc}: {lib().pnr_last_error().decode()}")
 
 
 def dptr(t, name="tensor"):

@@ -2,7 +2,7 @@
 
 The default grad-mode path on CUDA (`PNR_FUSED_BACKWARD` unset / auto / 2): `NeRFRenderer.forward` becomes ONE autograd
 node whose forward is the fused `pnr_render` (any engine, incl. the tensor engine) and whose backward is
-`pnr_render_backward` (fp32 recompute-in-backward).  Validated on B200 against the composed-torch path on the same
+`pnr_render_backward` (fp32 recompute-in-backward).  Validated on H100 against the composed-torch path on the same
 device and against the gradients the reference computed itself (tests/test_gpu_backward.py), and on the host emulator
 (tests/test_emu_kernels.py).
 

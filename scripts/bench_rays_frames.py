@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """HBM roofline of the two caller-side kernels (SURVEY 8f-3): pnr_gen_rays writes 32 B per ray, pnr_frames_u8 reads
-4 B and writes 1 B per value.  Buffers are larger than the 126 MB L2; CUDA events, median of 20 after 3 warm-ups."""
+4 B and writes 1 B per value.  Buffers are larger than the 50 MB L2; CUDA events, median of 20 after 3 warm-ups."""
 import json
 import os
 import sys

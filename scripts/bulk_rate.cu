@@ -1,4 +1,4 @@
-// Micro-benchmark: L2 -> shared-memory cp.async.bulk streaming (16 KB copies) with all 148 SMs reading the SAME
+// Micro-benchmark: L2 -> shared-memory cp.async.bulk streaming (16 KB copies) with all 132 SMs reading the SAME
 // 10 MB weight image (as the tensor engine does), N slots in flight per SM.  Reports cycles per copy.
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -34,7 +34,7 @@ __global__ void __launch_bounds__(64, 1) k_stream(const uint8_t* src, size_t src
 }
 
 template <int N>
-void run(const uint8_t* src, size_t bytes, int stagger, int grid = 148) {
+void run(const uint8_t* src, size_t bytes, int stagger, int grid = 132) {
   long long* d; cudaMalloc(&d, 8);
   auto kern = k_stream<N>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, N * 16384);

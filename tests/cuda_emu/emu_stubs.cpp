@@ -1,4 +1,4 @@
-// TEST INFRASTRUCTURE: the tensor-engine entry points are not emulated (tcgen05 has no host meaning); the emulated
+// TEST INFRASTRUCTURE: the tensor-engine entry points are not emulated (wgmma has no host meaning); the emulated
 // library reports the tensor engine as unavailable so that every call takes the SIMT path.
 #include <vector>
 
@@ -18,7 +18,7 @@ int tc_render(const PnrScene&, const PnrMlp&, const PnrMlp&, const float*, const
   set_error("tensor engine is not available in the emulator build");
   return PNR_ERR_UNSUPPORTED;
 }
-// the backward's GEMMs run on the fp32 SIMT SGEMM in the emulator (the tcgen05 GEMM has no host meaning)
+// the backward's GEMMs run on the fp32 SIMT SGEMM in the emulator (the wgmma GEMM has no host meaning)
 int sgemm(const float* A, int lda, const float* W, const float* bias, float* C, int ldc, int M, int N, int K, bool relu_a,
           bool accum, cudaStream_t s);
 int gemm_bf16x3(const float* A, int lda, const float* W, int ldw, const float* bias, float* C, int ldc, int M, int N, int K,

@@ -1,4 +1,4 @@
-"""Test infrastructure for the drop-in tests: the overlay tree (scripts/install_ref.py), a tiny SRN-format dataset on
+"""Test infrastructure for the drop-in tests: the overlay tree (oracle/install_ref.py), a tiny SRN-format dataset on
 disk, and a conf that switches the ImageNet download off.  The reference scripts themselves run UNMODIFIED."""
 import importlib.util
 import os
@@ -18,11 +18,11 @@ def _load(name, path):
     return mod
 
 
-install_ref = _load("pnr_install_ref", os.path.join(ROOT, "scripts", "install_ref.py"))
+install_ref = _load("pnr_install_ref", os.path.join(ROOT, "oracle", "install_ref.py"))
 
 
 def reference_root():
-    """The reference checkout for tests: /root/reference here, baseline/_ref on the GPU box; None if neither."""
+    """The reference checkout for tests: /root/reference here, oracle/_ref on the GPU box; None if neither."""
     return install_ref.find_reference()
 
 

@@ -1,7 +1,6 @@
 """TEST INFRASTRUCTURE: runs the UNMODIFIED reference in its own interpreter (its packages are called `model`, `render`,
 `util` like this repo's, so the two cannot share one) and dumps what a test needs into a .pt file.
 
-  python tests/ref_probe.py encoder <out.pt>      SpatialEncoder / encode() state on a small scene  (SURVEY 8a row a19)
   python tests/ref_probe.py checkpoint <dir>      a checkpoint written by the reference's own save_weights (row f-4)
   python tests/ref_probe.py load <dir>            the reference strict-loads <dir>/ours/pixel_nerf_latest (written by us)
 """
@@ -25,33 +24,6 @@ def scene(seed, SB, NS, H, W):
     focal = torch.rand(SB, 2, generator=g) * 50 + 40
     c = torch.rand(SB, 2, generator=g) * 4 + torch.tensor([W / 2.0, H / 2.0])
     return images, poses, focal, c
-
-
-def cmd_encoder(out):
-    model, _, _ = rh.import_reference()
-    res = {}
-    for name, use_first_pool, (SB, NS, H, W) in (("pool", True, (2, 2, 48, 64)), ("nopool", False, (1, 3, 40, 40))):
-        torch.manual_seed(3)
-        net = model.make_model(rh.model_conf(64, use_first_pool)).eval()
-        # BatchNorm running stats away from their (0, 1) initial values so that eval-mode BN does real work
-        with torch.no_grad():
-            for m in net.encoder.modules():
-                if isinstance(m, torch.nn.BatchNorm2d):
-                    m.running_mean.normal_(0, 0.1)
-                    m.running_var.uniform_(0.5, 1.5)
-        images, poses, focal, c = scene(7, SB, NS, H, W)
-        with torch.no_grad():
-            net.encode(images, poses, focal, c=c)
-            xyz = torch.randn(SB, 33, 3) * 0.5
-            dirs = torch.nn.functional.normalize(torch.randn(SB, 33, 3), dim=-1)
-            uv = torch.rand(SB * NS, 33, 2) * torch.tensor([W * 1.2, H * 1.2]) - 3.0
-            idx = net.encoder.index(uv, None, net.image_shape)
-        res[name] = dict(state_dict=net.state_dict(), images=images, poses=poses, focal=focal, c=c,
-                         use_first_pool=use_first_pool, latent=net.encoder.latent.clone(),
-                         latent_scaling=net.encoder.latent_scaling.clone(), poses_state=net.poses.clone(),
-                         focal_state=net.focal.clone(), c_state=net.c.clone(), image_shape=net.image_shape.clone(),
-                         uv=uv, index=idx, num_views_per_obj=net.num_views_per_obj)
-    torch.save(res, out)
 
 
 class _Args:
@@ -101,7 +73,7 @@ def cmd_load(d):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("cmd", choices=["encoder", "checkpoint", "load"])
+    ap.add_argument("cmd", choices=["checkpoint", "load"])
     ap.add_argument("out")
     a = ap.parse_args()
-    {"encoder": cmd_encoder, "checkpoint": cmd_checkpoint, "load": cmd_load}[a.cmd](a.out)
+    {"checkpoint": cmd_checkpoint, "load": cmd_load}[a.cmd](a.out)

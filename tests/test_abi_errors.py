@@ -7,7 +7,7 @@ import os
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "pixel-nerf_b200", "lib", "libpnr_sm100.so")
+LIB = os.path.join(ROOT, "pixel-nerf_b200", "lib", "libpnr_sm90.so")
 
 
 @pytest.fixture(scope="module")

@@ -23,7 +23,7 @@ def test_header_declares_the_documented_surface():
 
 def test_library_exports_every_declared_symbol():
     import __graft_entry__ as ge
-    lib_path = os.path.join(ROOT, "pixel-nerf_b200", "lib", "libpnr_sm100.so")
+    lib_path = os.path.join(ROOT, "pixel-nerf_b200", "lib", "libpnr_sm90.so")
     if not os.path.exists(lib_path):
         ge.build()
     lib = ctypes.CDLL(lib_path)

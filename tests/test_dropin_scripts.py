@@ -1,5 +1,5 @@
 """north_star: "eval/gen_video.py and train/train.py drop in unchanged".  The reference's scripts start with
-`sys.path.insert(0, <script dir>/../src)`, so the supported install is the overlay tree of scripts/install_ref.py
+`sys.path.insert(0, <script dir>/../src)`, so the supported install is the overlay tree of oracle/install_ref.py
 (the reference's eval/ train/ conf/ next to THIS package's src/).  These CPU tests execute the UNMODIFIED scripts'
 module tops (all their imports, then `util.args.parse_args` -> `--help`) against the overlay, and check which files the
 names resolve to.  Running the scripts' main loops needs a GPU: tests/test_gpu_dropin_scripts.py."""
@@ -13,7 +13,7 @@ import dropin_util as du
 
 SCRIPTS = ["train/train.py", "eval/gen_video.py", "eval/eval.py", "eval/eval_approx.py", "eval/eval_real.py"]
 
-needs_ref = pytest.mark.skipif(du.reference_root() is None, reason="no reference checkout (/root/reference or baseline/_ref)")
+needs_ref = pytest.mark.skipif(du.reference_root() is None, reason="no reference checkout (/root/reference or oracle/_ref)")
 
 
 @needs_ref

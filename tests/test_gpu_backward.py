@@ -135,7 +135,7 @@ def test_gemm_nt_fp16_split_engine():
                                                (777, 130, 48, False, True)])     # ragged N, one k-step
 def test_gemm_nt_engines(M, N, K, relu, accum, engine):
     """pnr_gemm_nt (the contraction of the backward path) against a float64 product: the fp32 FFMA engine to fp32
-    rounding, the split-bf16 tcgen05 engine to 16-bit-mantissa operands (<= 3e-5 of the row/column scale)."""
+    rounding, the split-bf16 wgmma engine to 16-bit-mantissa operands (<= 3e-5 of the row/column scale)."""
     import gpu_util  # noqa: F401
     import pnr_native as pn
     dev = torch.device("cuda:0")

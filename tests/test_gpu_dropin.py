@@ -19,6 +19,7 @@ def test_gen_video_call_sequence():
     from model import make_model
     from render import NeRFRenderer
 
+    torch.manual_seed(0)                                 # the scene must not depend on which tests ran before
     conf = util.hocon.parse_file(os.path.join(PKG, "conf", "exp", "srn.conf"))
     conf.put("model.encoder.pretrained", False)          # no network in the test image
     device = util.get_cuda(0)

@@ -1,4 +1,4 @@
-"""GPU parity of the tensor engine (tcgen05 split-fp16 fused kernel) against the CPU oracle.
+"""GPU parity of the tensor engine (wgmma split-fp16 fused kernel) against the CPU oracle.
 Tolerance on RGB is the north-star 1e-4; sigma (unbounded) is compared relatively."""
 import pytest
 import torch

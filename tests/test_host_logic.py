@@ -58,19 +58,18 @@ def _flatten(c, prefix=""):
 
 def test_shipped_confs_equal_the_reference_confs():
     """Every exp conf and expconf.conf of this package parses to the same tree as the reference's own file (read with
-    the same in-repo HOCON reader; the reference's files are the schema)."""
-    ref = None
-    for root in (os.environ.get("PIXELNERF_REF"), "/root/reference", os.path.join(ROOT, "baseline", "_ref")):
-        if root and os.path.isdir(os.path.join(root, "conf", "exp")):
-            ref = root
-            break
-    if ref is None:
-        pytest.skip("no reference checkout")
-    for name in sorted(os.listdir(os.path.join(ref, "conf", "exp"))):
-        ours = hocon.parse_file(os.path.join(PKG, "conf", "exp", name))
-        theirs = hocon.parse_file(os.path.join(ref, "conf", "exp", name))
-        assert _flatten(ours) == _flatten(theirs), name
-    assert _flatten(hocon.parse_file(os.path.join(PKG, "expconf.conf"))) == _flatten(hocon.parse_file(os.path.join(ref, "expconf.conf")))
+    the same in-repo HOCON reader; the reference's files are the schema).  The reference's trees are stored in
+    tests/golden/ref_confs.json (oracle/make_golden.py --only confs)."""
+    import json
+    with open(os.path.join(gu.GOLD, "ref_confs.json")) as f:
+        ref = json.load(f)
+    ours = {"exp/" + name: _flatten(hocon.parse_file(os.path.join(PKG, "conf", "exp", name)))
+            for name in sorted(os.listdir(os.path.join(PKG, "conf", "exp")))}
+    ours["expconf.conf"] = _flatten(hocon.parse_file(os.path.join(PKG, "expconf.conf")))
+    ours = json.loads(json.dumps(ours))       # the stored trees went through JSON (tuples -> lists)
+    assert sorted(ours) == sorted(ref)
+    for name in ref:
+        assert ours[name] == ref[name], name
 
 
 def test_model_state_dict_keys_and_shapes():

@@ -1,10 +1,11 @@
-"""State producer and checkpoint compatibility against the UNMODIFIED reference (run in its own interpreter by
-tests/ref_probe.py):
+"""State producer and checkpoint compatibility against the UNMODIFIED reference:
 
   * a19: `SpatialEncoder.forward` / `PixelNeRFNet.encode` -- same state_dict, same images -> the same latent, camera
-    state and `index()` values as the reference (src/model/encoder.py:111-164, src/model/models.py:89-144);
+    state and `index()` values as the reference (src/model/encoder.py:111-164, src/model/models.py:89-144); the
+    reference's outputs are stored in tests/golden/encode_state.npz (oracle/make_golden.py);
   * f-4: a checkpoint written by the reference's own `save_weights` strict-loads here and gives the reference's field
-    values; a checkpoint written here strict-loads in the reference (src/model/models.py:268-316).
+    values; a checkpoint written here strict-loads in the reference (src/model/models.py:268-316).  This one runs the
+    reference itself (in its own interpreter, tests/ref_probe.py) and needs a checkout.
 """
 import os
 import subprocess
@@ -17,7 +18,7 @@ import dropin_util as du
 import gpu_util
 
 PROBE = os.path.join(du.ROOT, "tests", "ref_probe.py")
-needs_ref = pytest.mark.skipif(du.reference_root() is None, reason="no reference checkout (/root/reference or baseline/_ref)")
+needs_ref = pytest.mark.skipif(du.reference_root() is None, reason="no reference checkout (/root/reference or oracle/_ref)")
 
 
 def probe(*argv):
@@ -33,28 +34,33 @@ class Args:
         self.checkpoints_path, self.name, self.resume = d, name, resume
 
 
-@needs_ref
-def test_encoder_and_encode_state_match_the_reference(tmp_path):
-    out = str(tmp_path / "enc.pt")
-    probe("encoder", out)
-    cases = torch.load(out)
+def test_encoder_and_encode_state_match_the_reference():
+    import numpy as np
+    from golden_util import GOLD, oracle
     from model import make_model
-    for name, ref in cases.items():
-        net = make_model(gpu_util.model_conf(64, ref["use_first_pool"])).eval()
-        missing = net.load_state_dict(ref["state_dict"], strict=True)
+    z = np.load(os.path.join(GOLD, "encode_state.npz"))
+    for name, (use_first_pool, (SB, NS, H, W)) in oracle.ENCODE_CASES.items():
+        ref = lambda k: torch.from_numpy(np.asarray(z[name + "/" + k]))
+        net = make_model(gpu_util.model_conf(64, use_first_pool)).eval()
+        missing = net.load_state_dict(oracle.seeded_state(net.state_dict(), 3), strict=True)
         assert not missing.missing_keys and not missing.unexpected_keys
+        images, poses, focal, c, uv = oracle.encode_scene(7, SB, NS, H, W)
         with torch.enable_grad():     # CPU tensors: the composed-torch path (encode() itself has no fused part)
-            net.encode(ref["images"], ref["poses"], ref["focal"], c=ref["c"])
-            idx = net.encoder.index(ref["uv"], None, net.image_shape)
+            net.encode(images, poses, focal, c=c)
+            idx = net.encoder.index(uv, None, net.image_shape)
         lat = net.encoder.latent.detach()
-        assert lat.shape == ref["latent"].shape, name
-        assert (lat - ref["latent"]).abs().max() <= 1e-6 * ref["latent"].abs().max(), name
-        assert torch.equal(net.encoder.latent_scaling, ref["latent_scaling"])
-        assert torch.equal(net.poses, ref["poses_state"])
-        assert torch.equal(net.focal, ref["focal_state"]) and torch.equal(net.c, ref["c_state"])
-        assert torch.equal(net.image_shape, ref["image_shape"])
-        assert net.num_views_per_obj == ref["num_views_per_obj"]
-        assert (idx.detach() - ref["index"]).abs().max() <= 1e-5 * ref["index"].abs().max()
+        assert list(lat.shape) == ref("latent_shape").tolist(), name
+        lat_s = lat.reshape(-1)[oracle.encode_sample_index(lat.numel(), 1)]
+        assert (lat_s - ref("latent")).abs().max() <= 1e-6 * ref("latent_absmax"), name
+        assert torch.equal(net.encoder.latent_scaling, ref("latent_scaling"))
+        assert torch.equal(net.poses, ref("poses"))
+        assert torch.equal(net.focal, ref("focal")) and torch.equal(net.c, ref("c"))
+        assert torch.equal(net.image_shape, ref("image_shape"))
+        assert net.num_views_per_obj == int(ref("num_views_per_obj"))
+        idx = idx.detach()
+        assert list(idx.shape) == ref("index_shape").tolist(), name
+        idx_s = idx.reshape(-1)[oracle.encode_sample_index(idx.numel(), 2)]
+        assert (idx_s - ref("index")).abs().max() <= 1e-5 * ref("index_absmax"), name
 
 
 @needs_ref

@@ -120,6 +120,17 @@ typedef struct PnrRenderOut {
   float* z_fine;         /* [R][Kc+Kf]  sorted merged samples (nerf.py:294-295) */
 } PnrRenderOut;
 
+/* Upstream gradients of a loss w.r.t. the six differentiable outputs of NeRFRenderer.forward (nerf.py:251-316), shapes
+ * as in PnrRenderOut.  Any pointer may be NULL, meaning a zero gradient (the loss does not use that output). */
+typedef struct PnrRenderGrad {
+  const float* d_rgb_coarse;     /* [R][3]      */
+  const float* d_depth_coarse;   /* [R]         */
+  const float* d_weights_coarse; /* [R][Kc]     */
+  const float* d_rgb_fine;       /* [R][3]      */
+  const float* d_depth_fine;     /* [R]         */
+  const float* d_weights_fine;   /* [R][Kc+Kf]  */
+} PnrRenderGrad;
+
 int pnr_abi_version(void);
 const char* pnr_last_error(void);
 
@@ -175,18 +186,38 @@ int pnr_field_backward(const PnrScene* scene, const PnrMlp* mlp, const float* xy
                        const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz, int64_t P,
                        void* workspace, size_t workspace_bytes, void* stream);
 
-/* Backward of pnr_render for a loss on the two rgb outputs (train/train.py:199-215: MSE coarse + MSE fine), i.e. what
- * loss.backward() does below `render_par(all_rays, want_weights=True)`:
+/* Backward of the compositing tail (pnr_composite; oracle/pnr_aux_backward.py::composite_backward): upstream gradients
+ * d_rgb [R][3], d_depth [R], d_weights [R][K] (each may be NULL = zero) ->
+ *   d_field [R][K][4] w.r.t. (sigmoid rgb, relu sigma), d_z [R][K] w.r.t. the sample depths (both overwritten).
+ * d_z is the compositing's own term only (deltas and depth); the positions' share (points = o + z d) is not in it. */
+int pnr_composite_backward(const float* rays, const float* z, const float* field, int32_t white_bkgd,
+                           const float* d_rgb, const float* d_depth, const float* d_weights, float* d_field,
+                           float* d_z, int64_t R, int32_t K, void* stream);
+
+/* Backward of pnr_render for a loss on any of its outputs, i.e. what loss.backward() does below
+ * `render_par(all_rays, want_weights=True)` (train/train.py:199-215, plus e.g. the alpha loss of model/loss.py on
+ * fine.weights.sum(-1), or a depth loss):
  *   fwd          : the forward call's outputs that the backward needs: z_coarse, z_fine (sorted), depth_coarse
- *   d_rgb_*      : [SB*B][3] upstream gradients (d_rgb_fine NULL when n_fine == 0)
+ *   up           : upstream gradients of the six outputs (NULL = all zero); a pass whose three gradients are all
+ *                  NULL is skipped
  *   grad_*       : writable PnrMlp-shaped gradient buffers, accumulated (+=); grad_fine NULL when mlp_fine is NULL
  *   d_latent_nhwc: [V][Hl][Wl][C], accumulated (+=); may be NULL
  * The coarse weights are detached for importance sampling but the coarse depth is not (nerf.py:286-291), so the fine
- * loss also reaches the coarse MLP.  Gradients w.r.t. the depth / weights outputs are not supported.
- * Arithmetic = oracle/pnr_backward.py::train_loss_backward; validated on H100 against the reference's own gradients.
+ * outputs' gradients also reach the coarse MLP: d(depth_coarse) = up->d_depth_coarse + the depth-centred samples' share.
+ * Arithmetic = oracle/pnr_aux_backward.py::render_backward.  Same workspace as pnr_render_backward.
  * This is the backward of the default CUDA training path (NeRFRenderer.forward in grad mode). */
 size_t pnr_render_backward_workspace_bytes(const PnrScene* scene, const PnrMlp* mlp_coarse,
                                            const PnrMlp* mlp_fine, const PnrRenderCfg* cfg, int64_t B);
+int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                           const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise,
+                           const PnrRenderOut* fwd, const PnrRenderGrad* up, const PnrMlp* grad_coarse,
+                           const PnrMlp* grad_fine, float* d_latent_nhwc, int64_t B, void* workspace,
+                           size_t workspace_bytes, void* stream);
+
+/* pnr_render_backward_ex for a loss on the two rgb outputs only (train/train.py:199-215: MSE coarse + MSE fine):
+ *   d_rgb_*      : [SB*B][3] upstream gradients, required (d_rgb_fine NULL when n_fine == 0)
+ * Gradients w.r.t. the depth / weights outputs are not supported by this entry point; use pnr_render_backward_ex.
+ * Arithmetic = oracle/pnr_backward.py::train_loss_backward; validated on H100 against the reference's own gradients. */
 int pnr_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
                         const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise,
                         const PnrRenderOut* fwd, const float* d_rgb_coarse, const float* d_rgb_fine,

@@ -288,11 +288,10 @@ size_t pnr_render_backward_workspace_bytes(const PnrScene* scene, const PnrMlp* 
   return b + f + 4096;
 }
 
-int pnr_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
-                        const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise, const PnrRenderOut* fwd,
-                        const float* d_rgb_coarse, const float* d_rgb_fine, const PnrMlp* grad_coarse,
-                        const PnrMlp* grad_fine, float* d_latent_nhwc, int64_t B, void* workspace,
-                        size_t workspace_bytes, void* stream) {
+// argument checks shared by pnr_render_backward and pnr_render_backward_ex, in the order the former always made them
+static int check_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                                 const PnrRenderCfg* cfg, const PnrNoise* noise, const PnrRenderOut* fwd,
+                                 const PnrMlp* grad_coarse, const PnrMlp* grad_fine, int64_t B) {
   int rc;
   if ((rc = check_scene(scene))) return rc;
   if ((rc = check_mlp(mlp_coarse))) return rc;
@@ -304,12 +303,26 @@ int pnr_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const P
                     cfg->n_fine_depth <= cfg->n_fine,
                 "bad sample counts");
   PNR_CHECK_ARG(B >= 0, "B must be >= 0");
+  return PNR_OK;
+}
+
+int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                           const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise, const PnrRenderOut* fwd,
+                           const PnrRenderGrad* up, const PnrMlp* grad_coarse, const PnrMlp* grad_fine,
+                           float* d_latent_nhwc, int64_t B, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc;
+  if ((rc = check_render_backward(scene, mlp_coarse, mlp_fine, cfg, noise, fwd, grad_coarse, grad_fine, B))) return rc;
   const int64_t R = B * scene->SB;
   if (R == 0) return PNR_OK;
   const int Kc = cfg->n_coarse, Kf = cfg->n_fine, Kfd = cfg->n_fine_depth, K = Kc + Kf;
-  PNR_CHECK_ARG(rays && workspace && d_rgb_coarse && fwd->z_coarse, "NULL pointer (rays, workspace, d_rgb_coarse, z_coarse)");
-  if (Kf > 0) PNR_CHECK_ARG(d_rgb_fine && fwd->z_fine, "fine pass needs d_rgb_fine and the forward's z_fine");
-  if (Kf > 0 && Kfd > 0) PNR_CHECK_ARG(fwd->depth_coarse && noise->n_depth, "depth samples need depth_coarse and n_depth");
+  const PnrRenderGrad g = up ? *up : PnrRenderGrad{};
+  // a pass whose outputs all have a NULL (zero) gradient contributes nothing and is skipped
+  const bool fine_grad = Kf > 0 && (g.d_rgb_fine || g.d_depth_fine || g.d_weights_fine);
+  const bool depth_path = fine_grad && Kfd > 0;
+  const bool coarse_grad = g.d_rgb_coarse || g.d_depth_coarse || g.d_weights_coarse || depth_path;
+  PNR_CHECK_ARG(rays && workspace && fwd->z_coarse, "NULL pointer (rays, workspace, z_coarse)");
+  if (fine_grad) PNR_CHECK_ARG(fwd->z_fine, "fine-pass gradients need the forward's z_fine");
+  if (depth_path) PNR_CHECK_ARG(fwd->depth_coarse && noise->n_depth, "depth samples need depth_coarse and n_depth");
   if (workspace_bytes < pnr_render_backward_workspace_bytes(scene, mlp_coarse, mlp_fine, cfg, B)) {
     set_error("workspace too small: %zu < %zu", workspace_bytes,
               pnr_render_backward_workspace_bytes(scene, mlp_coarse, mlp_fine, cfg, B));
@@ -324,37 +337,68 @@ int pnr_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const P
   float* d_depth = ar.take<float>((size_t)R);
   char* rest = ar.base + align_up(ar.off, 256);
   const size_t rest_bytes = workspace_bytes - align_up(ar.off, 256);
-  const bool depth_path = Kf > 0 && Kfd > 0;
+  const float* d_depth_coarse = g.d_depth_coarse;
   PointSource src{};
   src.mode = 1;
   src.rays = rays;
-  if (Kf > 0) {   // fine pass first: it feeds d(depth_coarse) into the coarse pass (nerf.py:289-291)
+  if (fine_grad) {   // fine pass first: it feeds d(depth_coarse) into the coarse pass (nerf.py:289-291)
     const PnrMlp* m = mlp_fine ? mlp_fine : mlp_coarse;
-    const PnrMlp* g = mlp_fine ? grad_fine : grad_coarse;
+    const PnrMlp* gm = mlp_fine ? grad_fine : grad_coarse;
     src.z = fwd->z_fine;
     src.K = K;
     src.P = B * K;
     const float* pj = mlp_fine ? scene->proj_fine : scene->proj_coarse;
     if ((rc = field_dispatch(*scene, *m, pj, src, R * K, field, cfg->engine, rest, rest_bytes, s))) return rc;
-    if ((rc = launch_composite_bwd(rays, fwd->z_fine, field, d_rgb_fine, nullptr, cfg->white_bkgd, d_field, d_z, R, K, s)))
+    if ((rc = launch_composite_bwd(rays, fwd->z_fine, field, g.d_rgb_fine, g.d_depth_fine, g.d_weights_fine,
+                                   cfg->white_bkgd, d_field, d_z, R, K, s)))
       return rc;
-    if ((rc = field_backward(*scene, *m, src, R * K, d_field, *g, d_latent_nhwc, depth_path ? d_xyz : nullptr, rest,
+    if ((rc = field_backward(*scene, *m, src, R * K, d_field, *gm, d_latent_nhwc, depth_path ? d_xyz : nullptr, rest,
                              rest_bytes, s)))
       return rc;
-    if (depth_path &&
-        (rc = launch_depth_grad(rays, fwd->z_fine, fwd->depth_coarse, noise->n_depth, cfg->depth_std, d_z, d_xyz,
-                                d_depth, R, K, Kfd, s)))
-      return rc;
+    if (depth_path) {
+      if ((rc = launch_depth_grad(rays, fwd->z_fine, fwd->depth_coarse, noise->n_depth, cfg->depth_std, d_z, d_xyz,
+                                  g.d_depth_coarse, d_depth, R, K, Kfd, s)))
+        return rc;
+      d_depth_coarse = d_depth;
+    }
   }
+  if (!coarse_grad) return PNR_OK;
   src.z = fwd->z_coarse;
   src.K = Kc;
   src.P = B * Kc;
   if ((rc = field_dispatch(*scene, *mlp_coarse, scene->proj_coarse, src, R * Kc, field, cfg->engine, rest, rest_bytes, s)))
     return rc;
-  if ((rc = launch_composite_bwd(rays, fwd->z_coarse, field, d_rgb_coarse, depth_path ? d_depth : nullptr,
+  if ((rc = launch_composite_bwd(rays, fwd->z_coarse, field, g.d_rgb_coarse, d_depth_coarse, g.d_weights_coarse,
                                  cfg->white_bkgd, d_field, d_z, R, Kc, s)))
     return rc;
   return field_backward(*scene, *mlp_coarse, src, R * Kc, d_field, *grad_coarse, d_latent_nhwc, nullptr, rest, rest_bytes, s);
+}
+
+int pnr_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                        const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise, const PnrRenderOut* fwd,
+                        const float* d_rgb_coarse, const float* d_rgb_fine, const PnrMlp* grad_coarse,
+                        const PnrMlp* grad_fine, float* d_latent_nhwc, int64_t B, void* workspace,
+                        size_t workspace_bytes, void* stream) {
+  int rc;
+  if ((rc = check_render_backward(scene, mlp_coarse, mlp_fine, cfg, noise, fwd, grad_coarse, grad_fine, B))) return rc;
+  if (B * scene->SB == 0) return PNR_OK;
+  PNR_CHECK_ARG(rays && workspace && d_rgb_coarse && fwd->z_coarse, "NULL pointer (rays, workspace, d_rgb_coarse, z_coarse)");
+  if (cfg->n_fine > 0) PNR_CHECK_ARG(d_rgb_fine && fwd->z_fine, "fine pass needs d_rgb_fine and the forward's z_fine");
+  PnrRenderGrad up{};
+  up.d_rgb_coarse = d_rgb_coarse;
+  up.d_rgb_fine = cfg->n_fine > 0 ? d_rgb_fine : nullptr;
+  return pnr_render_backward_ex(scene, mlp_coarse, mlp_fine, cfg, rays, noise, fwd, &up, grad_coarse, grad_fine,
+                                d_latent_nhwc, B, workspace, workspace_bytes, stream);
+}
+
+int pnr_composite_backward(const float* rays, const float* z, const float* field, int32_t white_bkgd,
+                           const float* d_rgb, const float* d_depth, const float* d_weights, float* d_field, float* d_z,
+                           int64_t R, int32_t K, void* stream) {
+  PNR_CHECK_ARG(R >= 0 && K >= 1, "bad sizes");
+  if (R == 0) return PNR_OK;
+  PNR_CHECK_ARG(rays && z && field && d_field && d_z, "NULL pointer");
+  return launch_composite_bwd(rays, z, field, d_rgb, d_depth, d_weights, white_bkgd, d_field, d_z, R, K,
+                              (cudaStream_t)stream);
 }
 
 size_t pnr_render_workspace_bytes(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,

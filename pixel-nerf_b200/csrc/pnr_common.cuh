@@ -98,13 +98,14 @@ size_t simt_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int64_t total
 int simt_field_eval(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src, int64_t total_points,
                     float* out, void* ws, size_t ws_bytes, cudaStream_t s);
 
-// renderer backward pieces (pnr_stages.cu): compositing, z from positions, coarse depth through the depth samples
+// renderer backward pieces (pnr_stages.cu): compositing, z from positions, coarse depth through the depth samples.
+// d_rgb [R][3], d_depth [R], d_weights [R][K], d_depth_up [R] may each be NULL (zero).
 int launch_composite_bwd(const float* rays, const float* z, const float* field, const float* d_rgb,
-                         const float* d_depth, int white, float* d_field, float* d_z, int64_t R, int K,
-                         cudaStream_t s);
+                         const float* d_depth, const float* d_weights, int white, float* d_field, float* d_z,
+                         int64_t R, int K, cudaStream_t s);
 int launch_depth_grad(const float* rays, const float* z_sorted, const float* depth, const float* nd,
-                      float depth_std, float* d_z, const float* d_xyz, float* d_depth, int64_t R, int K, int Kfd,
-                      cudaStream_t s);
+                      float depth_std, float* d_z, const float* d_xyz, const float* d_depth_up, float* d_depth,
+                      int64_t R, int K, int Kfd, cudaStream_t s);
 
 // ---- field backward, SIMT first path (pnr_field_bwd.cu) --------------------------------
 size_t field_backward_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int64_t total_points);

@@ -242,20 +242,25 @@ int launch_frames_u8(const float* rgb, int64_t n, uint8_t* out, cudaStream_t s) 
 }
 
 // ----------------------------------------------------------------------------------------
-// Backward of the renderer's own arithmetic (oracle/pnr_backward.py::composite_backward and the sample plumbing of
-// train_loss_backward).  One thread per ray; two sweeps over the K samples instead of storing per-sample state:
-// sweep 1 accumulates S = sum_k g_k w_k, sweep 2 turns the running prefix into the transmittance suffix sums.
+// Backward of the renderer's own arithmetic (oracle/pnr_aux_backward.py::composite_backward / render_backward, which
+// extend oracle/pnr_backward.py's rgb-only formulas).  One thread per ray; two sweeps over the K samples instead of
+// storing per-sample state: sweep 1 accumulates S = sum_k g_k w_k, sweep 2 turns the running prefix into the transmittance suffix sums.
+// The per-sample weight gradient is g_k = d_rgb . c_k + d_depth z_k (- sum d_rgb on a white background) + d_weights_k;
+// any of the three upstream gradients may be NULL (zero).  Without d_weights the arithmetic is that of the rgb/depth-only
+// kernel bit for bit (the add is skipped, not done with 0).
 // ----------------------------------------------------------------------------------------
 __global__ void k_composite_bwd(const float* __restrict__ rays, const float* __restrict__ z,
                                 const float* __restrict__ field, const float* __restrict__ d_rgb,
-                                const float* __restrict__ d_depth, int white, float* __restrict__ d_field,
-                                float* __restrict__ d_z, int64_t R, int K) {
+                                const float* __restrict__ d_depth, const float* __restrict__ d_weights, int white,
+                                float* __restrict__ d_field, float* __restrict__ d_z, int64_t R, int K) {
   int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= R) return;
   const float far = rays[r * 8 + 7];
   const float* zr = z + r * K;
   const float4* fr = reinterpret_cast<const float4*>(field) + r * K;
-  const float gr = d_rgb[r * 3 + 0], gg = d_rgb[r * 3 + 1], gb = d_rgb[r * 3 + 2];
+  const float* dwr = d_weights ? d_weights + r * K : nullptr;
+  const float gr = d_rgb ? d_rgb[r * 3 + 0] : 0.f, gg = d_rgb ? d_rgb[r * 3 + 1] : 0.f,
+              gb = d_rgb ? d_rgb[r * 3 + 2] : 0.f;
   const float gd = d_depth ? d_depth[r] : 0.f;
   const float gbg = white ? (gr + gg + gb) : 0.f;   // rgb += 1 - sum w  (nerf.py:241-244)
   float S = 0.f;
@@ -265,7 +270,8 @@ __global__ void k_composite_bwd(const float* __restrict__ rays, const float* __r
       const float znext = (k + 1 < K) ? zr[k + 1] : far;
       const float4 f = fr[k];
       const float alpha = 1.0f - expf(-(znext - zk) * fmaxf(f.w, 0.f));
-      const float gw = ((gr * f.x + gg * f.y) + gb * f.z) + gd * zk - gbg;
+      float gw = ((gr * f.x + gg * f.y) + gb * f.z) + gd * zk - gbg;
+      if (dwr) gw += dwr[k];
       S += gw * (alpha * T);
       T = T * ((1.0f - alpha) + 1e-10f);
       zk = znext;
@@ -282,7 +288,8 @@ __global__ void k_composite_bwd(const float* __restrict__ rays, const float* __r
     const float alpha = 1.0f - e;
     const float t = (1.0f - alpha) + 1e-10f;
     const float w = alpha * T;
-    const float gw = ((gr * f.x + gg * f.y) + gb * f.z) + gd * zk - gbg;
+    float gw = ((gr * f.x + gg * f.y) + gb * f.z) + gd * zk - gbg;
+    if (dwr) gw += dwr[k];
     prefix += gw * w;
     const float d_a = gw * T - (S - prefix) / t;      // S - prefix = sum_{m>k} g_m w_m
     const float d_delta = d_a * e * sg;
@@ -298,10 +305,11 @@ __global__ void k_composite_bwd(const float* __restrict__ rays, const float* __r
 }
 
 int launch_composite_bwd(const float* rays, const float* z, const float* field, const float* d_rgb,
-                         const float* d_depth, int white, float* d_field, float* d_z, int64_t R, int K,
-                         cudaStream_t s) {
+                         const float* d_depth, const float* d_weights, int white, float* d_field, float* d_z,
+                         int64_t R, int K, cudaStream_t s) {
   if (R == 0) return PNR_OK;
-  k_composite_bwd<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(rays, z, field, d_rgb, d_depth, white, d_field, d_z, R, K);
+  k_composite_bwd<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(rays, z, field, d_rgb, d_depth, d_weights, white,
+                                                              d_field, d_z, R, K);
   PNR_LAUNCH_CHECK();
   return PNR_OK;
 }
@@ -318,9 +326,11 @@ __global__ void k_dz_from_dxyz(float* __restrict__ d_z, const float* __restrict_
 // Gradient of the coarse depth through the depth-centred fine samples (nerf.py:150-161, 289-295): each sample
 // z_j = clamp(depth + n_j * std, near, far) sits somewhere in the sorted merged row; its slot is recomputed with the
 // forward's rank rule (smaller values first, ties by original index, the depth samples being the last index group).
+// d_depth = d_depth_up (the caller's gradient of the coarse depth output; NULL = zero) + that contribution.
 __global__ void k_depth_grad(const float* __restrict__ rays, const float* __restrict__ z_sorted,
                              const float* __restrict__ depth, const float* __restrict__ nd, float depth_std,
-                             const float* __restrict__ d_z, float* __restrict__ d_depth, int64_t R, int K, int Kfd) {
+                             const float* __restrict__ d_z, const float* __restrict__ d_depth_up,
+                             float* __restrict__ d_depth, int64_t R, int K, int Kfd) {
   int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= R) return;
   const float near = rays[r * 8 + 6], far = rays[r * 8 + 7], d = depth[r];
@@ -345,16 +355,17 @@ __global__ void k_depth_grad(const float* __restrict__ rays, const float* __rest
     const int pos = lo + ((ub - lo) - n_eq_depth) + n_eq_before;
     if (pos >= 0 && pos < K) acc += d_z[r * K + pos];
   }
-  d_depth[r] = acc;
+  d_depth[r] = d_depth_up ? d_depth_up[r] + acc : acc;
 }
 
 int launch_depth_grad(const float* rays, const float* z_sorted, const float* depth, const float* nd,
-                      float depth_std, float* d_z, const float* d_xyz, float* d_depth, int64_t R, int K, int Kfd,
-                      cudaStream_t s) {
+                      float depth_std, float* d_z, const float* d_xyz, const float* d_depth_up, float* d_depth,
+                      int64_t R, int K, int Kfd, cudaStream_t s) {
   if (R == 0) return PNR_OK;
   k_dz_from_dxyz<<<(unsigned)((R * K + 255) / 256), 256, 0, s>>>(d_z, d_xyz, rays, R, K);
   PNR_LAUNCH_CHECK();
-  k_depth_grad<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(rays, z_sorted, depth, nd, depth_std, d_z, d_depth, R, K, Kfd);
+  k_depth_grad<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(rays, z_sorted, depth, nd, depth_std, d_z, d_depth_up, d_depth, R,
+                                                           K, Kfd);
   PNR_LAUNCH_CHECK();
   return PNR_OK;
 }

@@ -54,6 +54,11 @@ class PnrRenderOut(C.Structure):
                 ("rgb_fine", _fp), ("depth_fine", _fp), ("weights_fine", _fp), ("z_fine", _fp)]
 
 
+class PnrRenderGrad(C.Structure):
+    _fields_ = [("d_rgb_coarse", _fp), ("d_depth_coarse", _fp), ("d_weights_coarse", _fp),
+                ("d_rgb_fine", _fp), ("d_depth_fine", _fp), ("d_weights_fine", _fp)]
+
+
 class PnrShard(C.Structure):
     _fields_ = [("scene", C.POINTER(PnrScene)), ("mlp_coarse", C.POINTER(PnrMlp)), ("mlp_fine", C.POINTER(PnrMlp)),
                 ("noise", C.POINTER(PnrNoise)), ("workspace", _fp), ("workspace_bytes", C.c_size_t),
@@ -88,6 +93,11 @@ def declare(L):
     L.pnr_render_backward.argtypes = [P(PnrScene), P(PnrMlp), P(PnrMlp), P(PnrRenderCfg), vp, P(PnrNoise),
                                       P(PnrRenderOut), vp, vp, P(PnrMlp), P(PnrMlp), vp, i64, vp, sz, vp]
     L.pnr_render_backward.restype = C.c_int
+    L.pnr_render_backward_ex.argtypes = [P(PnrScene), P(PnrMlp), P(PnrMlp), P(PnrRenderCfg), vp, P(PnrNoise),
+                                         P(PnrRenderOut), P(PnrRenderGrad), P(PnrMlp), P(PnrMlp), vp, i64, vp, sz, vp]
+    L.pnr_render_backward_ex.restype = C.c_int
+    L.pnr_composite_backward.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, i32, vp]
+    L.pnr_composite_backward.restype = C.c_int
     L.pnr_render_workspace_bytes.argtypes = [P(PnrScene), P(PnrMlp), P(PnrMlp), P(PnrRenderCfg), i64]
     L.pnr_render_workspace_bytes.restype = sz
     L.pnr_render.argtypes = [P(PnrScene), P(PnrMlp), P(PnrMlp), P(PnrRenderCfg), vp, P(PnrNoise),

@@ -6,8 +6,11 @@ node whose forward is the fused `pnr_render` (any engine, incl. the tensor engin
 device and against the gradients the reference computed itself (tests/test_gpu_backward.py), and on the host emulator
 (tests/test_emu_kernels.py).
 
-Differentiable outputs: `coarse.rgb`, `fine.rgb` (what train/train.py:199-212 puts into the loss).  depth and
-weights are returned but carry no gradient here (the shipped losses do not use them; lambda_alpha = 0).
+Every returned output is differentiable, as in the reference: `rgb`, `depth` and (with `want_weights`) `weights` of
+both passes.  A loss may so add e.g. the alpha loss of model/loss.py on `fine.weights.sum(-1)` or a depth term to the
+rgb losses of train/train.py:199-212; the backward is `pnr_render_backward_ex` with the upstream gradient of each
+output.  Outputs the loss does not use reach the backward as None and go to the library as NULL, so an rgb-only step
+runs the same arithmetic as the rgb-only entry point `pnr_render_backward`.
 """
 import torch
 
@@ -44,17 +47,13 @@ class _FusedRender(torch.autograd.Function):
         ctx.fwd = (res.coarse.z.reshape(R, Kc), res.fine.z.reshape(R, Kc + Kf) if fine else None,
                    res.coarse.depth.reshape(R))
         outs = [res.coarse.rgb, res.coarse.depth]
-        nondiff = [res.coarse.depth]
         if want_weights:
             outs.append(res.coarse.weights)
-            nondiff.append(res.coarse.weights)
         if fine:
             outs += [res.fine.rgb, res.fine.depth]
-            nondiff.append(res.fine.depth)
             if want_weights:
                 outs.append(res.fine.weights)
-                nondiff.append(res.fine.weights)
-        ctx.mark_non_differentiable(*nondiff)
+        ctx.set_materialize_grads(False)     # unused outputs arrive as None -> NULL (zero) in PnrRenderGrad
         ctx.layout = (want_weights, fine)
         return tuple(outs)
 
@@ -67,12 +66,15 @@ class _FusedRender(torch.autograd.Function):
         dev = rays.device
         SB, B, _ = rays.shape
         R = SB * B
-        d_rgb_c = grads[0]
-        d_rgb_f = grads[3 if want_weights else 2] if fine else None
-        zero = lambda: torch.zeros(R, 3, dtype=torch.float32, device=dev)
-        d_rgb_c = zero() if d_rgb_c is None else d_rgb_c.reshape(R, 3).contiguous().float()
+        names =["d_rgb_coarse", "d_depth_coarse"] + (["d_weights_coarse"] if want_weights else [])
         if fine:
-            d_rgb_f = zero() if d_rgb_f is None else d_rgb_f.reshape(R, 3).contiguous().float()
+            names += ["d_rgb_fine", "d_depth_fine"] + (["d_weights_fine"] if want_weights else [])
+        widths = dict(d_rgb_coarse=3, d_depth_coarse=1, d_weights_coarse=Kc, d_rgb_fine=3, d_depth_fine=1,
+                      d_weights_fine=Kc + Kf)
+        up = {}          # the upstream tensors must outlive the library call
+        for name, gr in zip(names, grads):
+            if gr is not None:
+                up[name] = gr.reshape(R, widths[name]).to(torch.float32).contiguous()
         scene, mc, mf, keep = model._scene_struct(want_fine=fine)
         mlps = [model.mlp_coarse] + ([model.mlp_fine] if (fine and model.mlp_fine is not None) else [])
         gdicts, gstructs = [], []
@@ -97,13 +99,15 @@ class _FusedRender(torch.autograd.Function):
             fwd.z_fine = pn.dptr(z_f.contiguous())
         cfg = pn.PnrRenderCfg(Kc, Kf, Kfd, depth_std, 1 if white else 0, pn.ENGINES[model.engine])
         L = pn.lib()
+        ug = pn.PnrRenderGrad()
+        for name, t in up.items():
+            setattr(ug, name, pn.dptr(t, name))
         nbytes = L.pnr_render_backward_workspace_bytes(scene, mc, mf, cfg, B)
         ws = pn.workspace(dev, nbytes)
         with torch.cuda.device(dev):
-            pn.check(L.pnr_render_backward(scene, mc, mf, cfg, pn.dptr(rays, "rays"), noise, fwd,
-                                           pn.dptr(d_rgb_c), pn.dptr(d_rgb_f), gstructs[0],
-                                           gstructs[1] if len(gstructs) > 1 else None, pn.dptr(d_latent), B,
-                                           ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
+            pn.check(L.pnr_render_backward_ex(scene, mc, mf, cfg, pn.dptr(rays, "rays"), noise, fwd, ug, gstructs[0],
+                                              gstructs[1] if len(gstructs) > 1 else None, pn.dptr(d_latent), B,
+                                              ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
         g_latent = d_latent.permute(0, 3, 1, 2) if want_latent else None
         flat = []
         for mlp, g in zip(mlps, gdicts):

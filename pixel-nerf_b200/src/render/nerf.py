@@ -7,8 +7,8 @@ Inference with a PixelNeRFNet on CUDA runs the whole sample -> field -> composit
 resample -> field -> composite chain in one C-ABI call (`pnr_render`, include/pnr.h); the
 random draws are made here with torch, in the reference's order, and handed to the kernels,
 so a seeded run replays the reference's samples.  With autograd enabled (training) on CUDA the
-same fused forward runs inside one autograd node whose backward is `pnr_render_backward`
-(render/fused_train.py); a foreign `model` callable, CPU tensors in grad mode (host-logic
+same fused forward runs inside one autograd node whose backward is `pnr_render_backward_ex`
+(render/fused_train.py), differentiable in rgb, depth and weights like the reference; a foreign `model` callable, CPU tensors in grad mode (host-logic
 tests) or PNR_FUSED_BACKWARD=0 use the composed torch path below.
 
 Multi-GPU (`bind_parallel(net, gpus)`): the reference wraps a `DataParallel(dim=1)`, which
@@ -355,7 +355,7 @@ class NeRFRenderer(torch.nn.Module):
         if (mode in ("auto", "2") and rays.is_cuda and self._is_pixelnerf(model)
                 and not (self.training and self.noise_std > 0.0)):
             # training step on the GPU (train/train.py:199-215): ONE autograd node, pnr_render forward +
-            # pnr_render_backward (render/fused_train.py).  PNR_FUSED_BACKWARD=1 keeps the renderer in torch ops with a
+            # pnr_render_backward_ex (render/fused_train.py), gradients through every output.  PNR_FUSED_BACKWARD=1 keeps the renderer in torch ops with a
             # fused field node (model/fused_field.py); =0 is the composed-torch path the gradient tests compare with.
             from .fused_train import fused_render_train
             return fused_render_train(self, model, rays, want_weights)

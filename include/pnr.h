@@ -267,16 +267,51 @@ typedef struct PnrShard {         /* everything device i needs for its piece of 
   void* stream;                   /* stream on device i to enqueue on (NULL: the handle's own stream)                  */
 } PnrShard;
 
+/* Gradient mode (train/train.py with several --gpu_id): pnr_mgpu_render_backward is the backward of one pnr_mgpu_render
+ * call.  Each shard runs pnr_render_backward_ex on its own device from the samples its forward left there; shard 0
+ * accumulates into the caller's gradient buffers on device 0, every other shard into a zeroed gradient arena on its
+ * device, and one kernel on device 0 then adds the arenas into device 0's, in shard order: grad0 += g_1 + ... + g_{n-1}
+ * (read over NVLink where device 0 can address device i, else first copied into a device-0 staging buffer).
+ * Shards on the same device run one after another on one stream, in the forward and the backward alike: the tensor
+ * engine's fused launch needs the whole device. */
+typedef struct PnrShardGrad {     /* everything device i needs for its piece of a backward call (pointers on device i) */
+  const float* rays;              /* [SB][B_i][8] the rays the shard's forward rendered (rays_stage, or device 0's)   */
+  const float* z_coarse;          /* [SB*B_i][Kc] the forward's samples: pnr_mgpu_render keeps stage.z_coarse /      */
+  const float* z_fine;            /* [SB*B_i][Kc+Kf]  stage.z_fine / stage.depth_coarse on device i even when out0     */
+  const float* depth_coarse;      /* [SB*B_i]         does not ask for them (z_fine NULL when n_fine == 0)            */
+  float* up_stage;                /* SB*B_i*(8+2*Kc+Kf) floats: the shard's slices of up0 (unused: shard 0, SB == 1)   */
+  const PnrMlp* grad_coarse;      /* shards i > 0: writable gradient buffers inside `arena` (shard 0: grad_coarse0)   */
+  const PnrMlp* grad_fine;        /* NULL when mlp_fine is NULL                                                       */
+  float* d_latent_nhwc;           /* [V][Hl][Wl][C] inside `arena`; NULL when d_latent0_nhwc is NULL                  */
+  float* arena;                   /* i > 0: [arena_count] holding the three above, zeroed by the driver; i == 0: the  */
+  int64_t arena_count;            /*   device-0 arena holding grad_coarse0 / grad_fine0 / d_latent0, same offsets     */
+  float* arena_stage0;            /* [arena_count] on DEVICE 0, needed where pnr_mgpu_peer_load(h, i) == 0             */
+  void* workspace;                /* >= pnr_render_backward_workspace_bytes(scene, mlp_coarse, mlp_fine, cfg, B_i)    */
+  size_t workspace_bytes;
+  void* stream;                   /* stream on device i (NULL: the handle's own stream)                               */
+} PnrShardGrad;
+
 int pnr_mgpu_create(const int32_t* device_ids, int32_t n, PnrMgpu** out);   /* enables peer access towards device_ids[0] */
 int pnr_mgpu_destroy(PnrMgpu* h);
 int32_t pnr_mgpu_size(const PnrMgpu* h);
 int32_t pnr_mgpu_peer_store(const PnrMgpu* h, int32_t i);   /* 1 if device i can store into device 0's memory */
+int32_t pnr_mgpu_peer_load(const PnrMgpu* h, int32_t i);    /* 1 if device 0 can read device i's memory (i > 0) */
 /* dst[i] on device i  <-  src on device 0 (dst[0] ignored, NULL entries skipped); ordered after streams[0] (device 0)
  * and enqueued on streams[i] (NULL array / entry: the handle's own streams). */
 int pnr_mgpu_broadcast(PnrMgpu* h, const void* src, void* const* dst, size_t bytes, void* const* streams);
 /* rays0 [SB][B][8] and out0 (tensors [SB*B][...], NULL = not wanted) on device 0; shards[n]. */
 int pnr_mgpu_render(PnrMgpu* h, const PnrShard* shards, const PnrRenderCfg* cfg, const float* rays0,
                     const PnrRenderOut* out0, int64_t B, void* stream0);
+/* Backward of the pnr_mgpu_render call made with the same shards, cfg and B.  up0: upstream gradients on device 0,
+ * [SB*B][...] as out0 (NULL / NULL entries = zero); grad_coarse0, grad_fine0, d_latent0_nhwc: device 0's buffers,
+ * accumulated (+=) as in pnr_render_backward_ex.  On return every shard's stream is ordered after the reduction, so
+ * the caller may release the shard buffers; the caller's stream0 is ordered after everything. */
+int pnr_mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
+                             const PnrRenderCfg* cfg, const PnrRenderGrad* up0, const PnrMlp* grad_coarse0,
+                             const PnrMlp* grad_fine0, float* d_latent0_nhwc, int64_t B, void* stream0);
+/* The reduction step on its own: dst[j] += src[0][j] + src[1][j] + ... + src[n-1][j], added left to right, for
+ * j < count.  src: host array of n <= 63 device pointers readable from the current device. */
+int pnr_sum_into(float* dst, const float* const* src, int32_t n, int64_t count, void* stream);
 
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.

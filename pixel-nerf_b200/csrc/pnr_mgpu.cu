@@ -13,18 +13,23 @@
 // Shards are torch.chunk pieces of the ray axis, so the gathered ray order equals DataParallel's.  Everything is
 // asynchronous; the caller's stream on gpus[0] waits on per-shard events.  No NCCL: inside one process peer access
 // is the whole transport (bench.py's one-process-per-GPU launcher uses NCCL through torch.distributed instead).
+#include <stdint.h>
 #include <stdlib.h>
 
 #include <vector>
 
 #include "pnr_common.cuh"
 
+#define PNR_MGPU_MAX_SOURCES 63   // pnr_mgpu_create takes at most 64 devices: device 0 plus 63 sources
+
 struct PnrMgpu {
   std::vector<int> dev;
   std::vector<cudaStream_t> stream;   // per device (index 0 unused: device 0 work runs on the caller's stream)
   std::vector<cudaEvent_t> done;      // per device
   std::vector<char> peer_to_0;        // device i can address device 0's memory
+  std::vector<char> peer_from_0;      // device 0 can address device i's memory (the backward's reduction reads it)
   cudaEvent_t start;                  // recorded on the caller's stream of device 0
+  cudaEvent_t reduced;                // recorded on device 0 after the backward's reduction
 };
 
 namespace pnr {
@@ -42,6 +47,92 @@ static void chunk_bounds(int64_t B, int n, int i, int64_t* a, int64_t* b) {
   *b = *a + per < B ? *a + per : B;
 }
 
+// The stream each shard is enqueued on: shard 0 uses the caller's stream, shard i its requested stream (NULL: the
+// handle's own) -- except that shards on the same device all take the stream of the first shard there.  The tensor
+// engine's fused render kernel spins on flags set by other CTAs of the same launch (DESIGN.md 3.1), which is deadlock
+// free only while the whole persistent grid is resident; two such launches running at once on one GPU break that.
+template <class Requested>
+static std::vector<cudaStream_t> shard_streams(const PnrMgpu* h, cudaStream_t stream0, Requested requested) {
+  const int n = (int)h->dev.size();
+  std::vector<cudaStream_t> s(n);
+  for (int i = 0; i < n; ++i) {
+    s[i] = i == 0 ? stream0 : (requested(i) ? (cudaStream_t)requested(i) : h->stream[i]);
+    for (int j = 0; j < i; ++j)
+      if (h->dev[j] == h->dev[i]) {
+        s[i] = s[j];
+        break;
+      }
+  }
+  return s;
+}
+
+// dst[j] += src[0][j] + ... + src[n-1][j], left to right; float4 body when every pointer is 16-byte aligned
+struct SumSources {
+  const float* p[PNR_MGPU_MAX_SOURCES];
+};
+
+__global__ void k_sum_into(float* dst, SumSources src, int n, int64_t count, int vec) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t n4 = vec ? count / 4 : 0;
+  for (int64_t v = t; v < n4; v += stride) {
+    float4 a = reinterpret_cast<const float4*>(dst)[v];
+    for (int k = 0; k < n; ++k) {
+      const float4 b = reinterpret_cast<const float4*>(src.p[k])[v];
+      a.x += b.x;
+      a.y += b.y;
+      a.z += b.z;
+      a.w += b.w;
+    }
+    reinterpret_cast<float4*>(dst)[v] = a;
+  }
+  for (int64_t j = n4 * 4 + t; j < count; j += stride) {
+    float a = dst[j];
+    for (int k = 0; k < n; ++k) a += src.p[k][j];
+    dst[j] = a;
+  }
+}
+
+static int launch_sum_into(float* dst, const float* const* src, int n, int64_t count, cudaStream_t s) {
+  if (count == 0 || n == 0) return PNR_OK;
+  SumSources ss{};
+  bool vec = ((uintptr_t)dst & 15) == 0;
+  for (int k = 0; k < n; ++k) {
+    ss.p[k] = src[k];
+    vec = vec && ((uintptr_t)src[k] & 15) == 0;
+  }
+  const int64_t items = vec ? count / 4 : count;  // (the <= 3 floats of a float4 tail go to the first threads)
+  const int threads = 256;
+  int64_t blocks = (items + threads - 1) / threads;
+  if (blocks < 1) blocks = 1;
+  if (blocks > 132 * 8) blocks = 132 * 8;        // grid-stride beyond 8 blocks per H100 SM
+  k_sum_into<<<(unsigned)blocks, threads, 0, s>>>(dst, ss, n, count, vec ? 1 : 0);
+  PNR_LAUNCH_CHECK();
+  return PNR_OK;
+}
+
+// Pointer p (into arena a) and q (into arena b) sit at the same offset inside the first `count` floats, or are both NULL.
+static bool same_offset(const void* p, const float* a, const void* q, const float* b, int64_t count) {
+  if (!p || !q) return !p && !q;
+  const intptr_t op = ((intptr_t)p - (intptr_t)a), oq = ((intptr_t)q - (intptr_t)b);
+  return op == oq && op >= 0 && op % 4 == 0 && op / 4 < count;
+}
+
+// Every gradient buffer of the two PnrMlp sits at the same offset in its arena.
+static bool same_layout(const PnrMlp* x, const float* a, const PnrMlp* y, const float* b, int64_t count) {
+  if (!x || !y) return !x && !y;
+  if (x->n_blocks != y->n_blocks || x->combine_layer != y->combine_layer) return false;
+  bool ok = same_offset(x->lin_in_w, a, y->lin_in_w, b, count) && same_offset(x->lin_in_b, a, y->lin_in_b, b, count) &&
+            same_offset(x->lin_out_w, a, y->lin_out_w, b, count) && same_offset(x->lin_out_b, a, y->lin_out_b, b, count);
+  const int nb = x->n_blocks < PNR_MAX_BLOCKS ? x->n_blocks : PNR_MAX_BLOCKS;
+  for (int k = 0; k < nb && ok; ++k)
+    ok = same_offset(x->fc0_w[k], a, y->fc0_w[k], b, count) && same_offset(x->fc0_b[k], a, y->fc0_b[k], b, count) &&
+         same_offset(x->fc1_w[k], a, y->fc1_w[k], b, count) && same_offset(x->fc1_b[k], a, y->fc1_b[k], b, count);
+  for (int k = 0; k < nb && k < x->combine_layer && ok; ++k)
+    ok = same_offset(x->lin_z_w[k], a, y->lin_z_w[k], b, count) && same_offset(x->lin_z_b[k], a, y->lin_z_b[k], b, count);
+  return ok;
+}
+
 }  // namespace pnr
 
 using namespace pnr;
@@ -56,6 +147,7 @@ int pnr_mgpu_create(const int32_t* device_ids, int32_t n, PnrMgpu** out) {
   h->stream.assign(n, nullptr);
   h->done.assign(n, nullptr);
   h->peer_to_0.assign(n, 0);
+  h->peer_from_0.assign(n, 0);
   for (int i = 0; i < n; ++i) {
     if (cudaSetDevice(h->dev[i]) != cudaSuccess) {
       set_error("pnr_mgpu_create: cannot select device %d", h->dev[i]);
@@ -75,7 +167,17 @@ int pnr_mgpu_create(const int32_t* device_ids, int32_t n, PnrMgpu** out) {
     }
   }
   cudaSetDevice(h->dev[0]);
+  for (int i = 1; i < n; ++i) {
+    int can = 0;
+    cudaDeviceCanAccessPeer(&can, h->dev[0], h->dev[i]);
+    if (can) {
+      cudaError_t e = cudaDeviceEnablePeerAccess(h->dev[i], 0);
+      if (e == cudaSuccess || e == cudaErrorPeerAccessAlreadyEnabled) h->peer_from_0[i] = 1;
+      cudaGetLastError();
+    }
+  }
   cudaEventCreateWithFlags(&h->start, cudaEventDisableTiming);
+  cudaEventCreateWithFlags(&h->reduced, cudaEventDisableTiming);
   *out = h;
   return PNR_OK;
 }
@@ -93,6 +195,7 @@ int pnr_mgpu_destroy(PnrMgpu* h) {
   }
   cudaSetDevice(h->dev[0]);
   cudaEventDestroy(h->start);
+  cudaEventDestroy(h->reduced);
   delete h;
   return PNR_OK;
 }
@@ -101,6 +204,10 @@ int32_t pnr_mgpu_size(const PnrMgpu* h) { return h ? (int32_t)h->dev.size() : 0;
 
 int32_t pnr_mgpu_peer_store(const PnrMgpu* h, int32_t i) {
   return (h && i >= 0 && i < (int32_t)h->dev.size()) ? (i == 0 ? 1 : h->peer_to_0[i]) : 0;
+}
+
+int32_t pnr_mgpu_peer_load(const PnrMgpu* h, int32_t i) {
+  return (h && i >= 0 && i < (int32_t)h->dev.size()) ? (i == 0 ? 1 : h->peer_from_0[i]) : 0;
 }
 
 int pnr_mgpu_broadcast(PnrMgpu* h, const void* src, void* const* dst, size_t bytes, void* const* streams) {
@@ -140,6 +247,7 @@ int pnr_mgpu_render(PnrMgpu* h, const PnrShard* shards, const PnrRenderCfg* cfg,
   PNR_CHECK_ARG(SB >= 1, "shard 0 has no scene");
   const int Kc = cfg->n_coarse, K = cfg->n_coarse + cfg->n_fine;
   const bool fine = cfg->n_fine > 0;
+  const std::vector<cudaStream_t> streams = shard_streams(h, (cudaStream_t)stream0, [&](int i) { return shards[i].stream; });
   PNR_CUDA(cudaSetDevice(h->dev[0]));
   PNR_CUDA(cudaEventRecord(h->start, (cudaStream_t)stream0));
   int rc = PNR_OK;
@@ -152,7 +260,7 @@ int pnr_mgpu_render(PnrMgpu* h, const PnrShard* shards, const PnrRenderCfg* cfg,
     const PnrShard& sh = shards[i];
     PNR_CHECK_ARG(sh.scene && sh.mlp_coarse && sh.noise && sh.workspace, "incomplete shard");
     PNR_CHECK_ARG(sh.scene->SB == SB, "all shards must hold the same objects");
-    cudaStream_t s = i == 0 ? (cudaStream_t)stream0 : (sh.stream ? (cudaStream_t)sh.stream : h->stream[i]);
+    cudaStream_t s = streams[i];
     PNR_CUDA(cudaSetDevice(h->dev[i]));
     if (i > 0) PNR_CUDA(cudaStreamWaitEvent(s, h->start, 0));
     // rays of the shard: in place on device 0 for one object, else a (strided) peer copy into the shard's stage
@@ -177,10 +285,9 @@ int pnr_mgpu_render(PnrMgpu* h, const PnrShard* shards, const PnrRenderCfg* cfg,
         if (best_dep0) o.depth_coarse = best_dep0 + a;
       }
     }
+    // the samples stay in the stage when it has room for them, wanted by out0 or not: the backward reads them there
     if (!out0->weights_coarse) o.weights_coarse = nullptr;
-    if (!out0->z_coarse) o.z_coarse = nullptr;
     if (!out0->weights_fine) o.weights_fine = nullptr;
-    if (!out0->z_fine) o.z_fine = nullptr;
     rc = pnr_render(sh.scene, sh.mlp_coarse, sh.mlp_fine, cfg, rays_i, sh.noise, &o, Bi, sh.workspace, sh.workspace_bytes, s);
     if (rc) break;
     struct Item { float* dst; const float* src; int64_t w; };
@@ -201,6 +308,133 @@ int pnr_mgpu_render(PnrMgpu* h, const PnrShard* shards, const PnrRenderCfg* cfg,
   PNR_CUDA(cudaSetDevice(h->dev[0]));
   for (int i = 1; i < used; ++i) PNR_CUDA(cudaStreamWaitEvent((cudaStream_t)stream0, h->done[i], 0));
   return rc;
+}
+
+int pnr_sum_into(float* dst, const float* const* src, int32_t n, int64_t count, void* stream) {
+  PNR_CHECK_ARG(n >= 0 && n <= PNR_MGPU_MAX_SOURCES && count >= 0, "bad sizes");
+  if (n == 0 || count == 0) return PNR_OK;
+  PNR_CHECK_ARG(dst && src, "NULL argument");
+  for (int k = 0; k < n; ++k) PNR_CHECK_ARG(src[k], "NULL source");
+  return launch_sum_into(dst, src, n, count, (cudaStream_t)stream);
+}
+
+int pnr_mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
+                             const PnrRenderCfg* cfg, const PnrRenderGrad* up0, const PnrMlp* grad_coarse0,
+                             const PnrMlp* grad_fine0, float* d_latent0_nhwc, int64_t B, void* stream0) {
+  PNR_CHECK_ARG(h && shards && shard_grads && cfg && grad_coarse0, "NULL argument");
+  PNR_CHECK_ARG(B >= 0, "B must be >= 0");
+  PNR_CHECK_ARG(cfg->n_coarse >= 1 && cfg->n_fine >= 0, "bad sample counts");
+  DevGuard guard;
+  const int n = (int)h->dev.size();
+  const int SB = shards[0].scene ? shards[0].scene->SB : 0;
+  PNR_CHECK_ARG(SB >= 1, "shard 0 has no scene");
+  const int Kc = cfg->n_coarse, K = cfg->n_coarse + cfg->n_fine;
+  const bool fine = cfg->n_fine > 0;
+  // the six upstream gradients of up0 and their widths; a NULL one stays NULL (zero) on every shard
+  const PnrRenderGrad g0 = up0 ? *up0 : PnrRenderGrad{};
+  const float* PnrRenderGrad::*const fields[6] = {&PnrRenderGrad::d_rgb_coarse, &PnrRenderGrad::d_depth_coarse,
+                                                 &PnrRenderGrad::d_weights_coarse, &PnrRenderGrad::d_rgb_fine,
+                                                 &PnrRenderGrad::d_depth_fine, &PnrRenderGrad::d_weights_fine};
+  const int64_t widths[6] = {3, 1, Kc, 3, 1, K};
+  bool any_up = false;
+  for (int k = 0; k < 6; ++k) any_up = any_up || ((k < 3 || fine) && g0.*fields[k]);
+  // check every shard before anything is enqueued
+  const PnrShardGrad& sg0 = shard_grads[0];
+  int used = 0;
+  for (int i = 0; i < n; ++i) {
+    int64_t a, b;
+    chunk_bounds(B, n, i, &a, &b);
+    if (b - a <= 0) continue;
+    const PnrShard& sh = shards[i];
+    const PnrShardGrad& sg = shard_grads[i];
+    PNR_CHECK_ARG(sh.scene && sh.mlp_coarse && sh.noise, "incomplete shard");
+    PNR_CHECK_ARG(sh.scene->SB == SB, "all shards must hold the same objects");
+    PNR_CHECK_ARG(sg.rays && sg.z_coarse && sg.workspace, "incomplete shard gradient (rays, z_coarse, workspace)");
+    if (any_up && (i > 0 || SB > 1)) PNR_CHECK_ARG(sg.up_stage, "shard gradient needs an upstream staging buffer");
+    if (i > 0) {
+      PNR_CHECK_ARG(sg0.arena && sg0.arena_count > 0, "shard gradient 0 needs device 0's gradient arena");
+      PNR_CHECK_ARG(sg.arena && sg.arena_count == sg0.arena_count, "shard gradient needs an arena of device 0's size");
+      PNR_CHECK_ARG(sg.grad_coarse && (!sh.mlp_fine || sg.grad_fine), "incomplete shard gradient (grad_coarse / grad_fine)");
+      PNR_CHECK_ARG(same_layout(sg.grad_coarse, sg.arena, grad_coarse0, sg0.arena, sg0.arena_count) &&
+                        same_layout(sh.mlp_fine ? sg.grad_fine : nullptr, sg.arena,
+                                    sh.mlp_fine ? grad_fine0 : nullptr, sg0.arena, sg0.arena_count) &&
+                        same_offset(sg.d_latent_nhwc, sg.arena, d_latent0_nhwc, sg0.arena, sg0.arena_count),
+                    "shard gradient arena must have device 0's layout");
+      PNR_CHECK_ARG(h->peer_from_0[i] || sg.arena_stage0, "shard gradient needs a device-0 staging arena (no peer access)");
+    }
+    used = i + 1;
+  }
+  if (used == 0) return PNR_OK;
+  PNR_CHECK_ARG(used - 1 <= PNR_MGPU_MAX_SOURCES, "too many shards");
+  const std::vector<cudaStream_t> streams =
+      shard_streams(h, (cudaStream_t)stream0, [&](int i) { return shard_grads[i].stream; });
+  PNR_CUDA(cudaSetDevice(h->dev[0]));
+  PNR_CUDA(cudaEventRecord(h->start, (cudaStream_t)stream0));     // up0 is ready
+  for (int i = 0; i < used; ++i) {
+    int64_t a, b;
+    chunk_bounds(B, n, i, &a, &b);
+    const int64_t Bi = b - a;
+    if (Bi <= 0) continue;
+    const PnrShard& sh = shards[i];
+    const PnrShardGrad& sg = shard_grads[i];
+    cudaStream_t s = streams[i];
+    PNR_CUDA(cudaSetDevice(h->dev[i]));
+    if (i > 0) PNR_CUDA(cudaStreamWaitEvent(s, h->start, 0));
+    // the shard's slice of each upstream gradient: in place for shard 0 of one object, else a strided copy
+    PnrRenderGrad gi{};
+    float* stage = sg.up_stage;
+    for (int k = 0; k < 6; ++k) {
+      const float* src = (k < 3 || fine) ? g0.*fields[k] : nullptr;
+      if (!src) continue;
+      const int64_t w = widths[k];
+      if (i == 0 && SB == 1) {
+        gi.*fields[k] = src + a * w;
+        continue;
+      }
+      int rc = copy_rows(stage, Bi * w, src + a * w, B * w, Bi * w, SB, s);
+      if (rc) return rc;
+      gi.*fields[k] = stage;
+      stage += SB * Bi * w;
+    }
+    if (i > 0) PNR_CUDA(cudaMemsetAsync(sg.arena, 0, (size_t)sg.arena_count * 4, s));
+    PnrRenderOut fwd{};
+    fwd.z_coarse = const_cast<float*>(sg.z_coarse);
+    fwd.z_fine = const_cast<float*>(sg.z_fine);
+    fwd.depth_coarse = const_cast<float*>(sg.depth_coarse);
+    int rc = pnr_render_backward_ex(sh.scene, sh.mlp_coarse, sh.mlp_fine, cfg, sg.rays, sh.noise, &fwd, &gi,
+                                    i == 0 ? grad_coarse0 : sg.grad_coarse, i == 0 ? grad_fine0 : sg.grad_fine,
+                                    i == 0 ? d_latent0_nhwc : sg.d_latent_nhwc, Bi, sg.workspace, sg.workspace_bytes, s);
+    if (rc) return rc;
+    if (i > 0) PNR_CUDA(cudaEventRecord(h->done[i], s));
+  }
+  // device 0: grad0 += g_1 + ... + g_{used-1}, one launch over the arenas, shards in order
+  PNR_CUDA(cudaSetDevice(h->dev[0]));
+  cudaStream_t s0 = (cudaStream_t)stream0;
+  std::vector<const float*> src;
+  for (int i = 1; i < used; ++i) {
+    int64_t a, b;
+    chunk_bounds(B, n, i, &a, &b);
+    if (b - a <= 0) continue;
+    const PnrShardGrad& sg = shard_grads[i];
+    PNR_CUDA(cudaStreamWaitEvent(s0, h->done[i], 0));
+    if (h->peer_from_0[i]) {
+      src.push_back(sg.arena);                                   // read over NVLink by the reduction kernel
+    } else {
+      PNR_CUDA(cudaMemcpyPeerAsync(sg.arena_stage0, h->dev[0], sg.arena, h->dev[i], (size_t)sg.arena_count * 4, s0));
+      src.push_back(sg.arena_stage0);
+    }
+  }
+  if (src.empty()) return PNR_OK;
+  int rc = launch_sum_into(sg0.arena, src.data(), (int)src.size(), sg0.arena_count, s0);
+  if (rc) return rc;
+  // later work on the shards' streams waits for the reduction, so their arenas can be released once this returns
+  PNR_CUDA(cudaEventRecord(h->reduced, s0));
+  for (int i = 1; i < used; ++i) {
+    if (streams[i] == s0) continue;
+    PNR_CUDA(cudaSetDevice(h->dev[i]));
+    PNR_CUDA(cudaStreamWaitEvent(streams[i], h->reduced, 0));
+  }
+  return PNR_OK;
 }
 
 }  // extern "C"

@@ -65,6 +65,13 @@ class PnrShard(C.Structure):
                 ("rays_stage", _fp), ("stage", PnrRenderOut), ("stream", _fp)]
 
 
+class PnrShardGrad(C.Structure):
+    _fields_ = [("rays", _fp), ("z_coarse", _fp), ("z_fine", _fp), ("depth_coarse", _fp), ("up_stage", _fp),
+                ("grad_coarse", C.POINTER(PnrMlp)), ("grad_fine", C.POINTER(PnrMlp)), ("d_latent_nhwc", _fp),
+                ("arena", _fp), ("arena_count", C.c_int64), ("arena_stage0", _fp),
+                ("workspace", _fp), ("workspace_bytes", C.c_size_t), ("stream", _fp)]
+
+
 _lib = None
 
 
@@ -117,7 +124,13 @@ def declare(L):
         L.pnr_mgpu_peer_store.restype = i32
         L.pnr_mgpu_broadcast.argtypes = [vp, vp, P(vp), sz, P(vp)]
         L.pnr_mgpu_render.argtypes = [vp, P(PnrShard), P(PnrRenderCfg), vp, P(PnrRenderOut), i64, vp]
-        for name in ("pnr_mgpu_create", "pnr_mgpu_destroy", "pnr_mgpu_broadcast", "pnr_mgpu_render"):
+        L.pnr_mgpu_peer_load.argtypes = [vp, i32]
+        L.pnr_mgpu_peer_load.restype = i32
+        L.pnr_mgpu_render_backward.argtypes = [vp, P(PnrShard), P(PnrShardGrad), P(PnrRenderCfg), P(PnrRenderGrad),
+                                               P(PnrMlp), P(PnrMlp), vp, i64, vp]
+        L.pnr_sum_into.argtypes = [vp, P(vp), i32, i64, vp]
+        for name in ("pnr_mgpu_create", "pnr_mgpu_destroy", "pnr_mgpu_broadcast", "pnr_mgpu_render",
+                     "pnr_mgpu_render_backward", "pnr_sum_into"):
             getattr(L, name).restype = C.c_int
     L.pnr_gemm_nt.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.pnr_gemm_nt.restype = C.c_int

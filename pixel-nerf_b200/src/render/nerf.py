@@ -15,7 +15,8 @@ Multi-GPU (`bind_parallel(net, gpus)`): the reference wraps a `DataParallel(dim=
 re-broadcasts the whole module on every call; `_ShardedRender` instead keeps a `_SceneReplica`
 (peer copies of the already-derived device state) per extra GPU, refreshed only when
 encode()/weights change, and slices rays with torch.chunk semantics, so ray order in the
-gathered output is identical.
+gathered output is identical.  In grad mode the shards also run their own backward and their
+gradients are summed onto gpus[0] (render/fused_train.py).
 """
 import os
 import warnings
@@ -153,8 +154,12 @@ class _ShardedRender(torch.nn.Module):
     gpus[0] through peer memory.  GPUs other than gpus[0] render from a `_SceneReplica`; every GPU draws its samples
     from its own generator (as under DataParallel).
 
-    Gradient mode (train/train.py with several --gpu_id): the autograd graph lives on gpus[0], so the step runs there
-    alone (with a one-time warning) -- replicas hold detached copies and would drop the shards' gradients."""
+    Gradient mode (train/train.py with several --gpu_id): one autograd node on gpus[0] (render/fused_train.py,
+    `_ShardedFusedRender`) runs the same sharded forward and then `pnr_mgpu_render_backward`: every GPU differentiates
+    its own shard from the samples its forward left there, and one kernel on gpus[0] sums the shards' weight and latent
+    gradients onto gpus[0]'s, so autograd continues into the encoder there as under DataParallel.  The optimizer step
+    and encode() change the weights and the scene on every step, so every step refreshes the replicas.  Other models,
+    CPU rays or PNR_FUSED_BACKWARD=0/1 run the step on gpus[0] alone, with a one-time warning."""
 
     def __init__(self, wrapped, gpus):
         super().__init__()
@@ -163,6 +168,8 @@ class _ShardedRender(torch.nn.Module):
         self._replicas = {g: _SceneReplica(torch.device("cuda", g)) for g in self.gpus[1:]}
         self._warned = False
         self._handle = None
+        self._keep, self._keep_bwd = [], []
+        self.timing = None          # dict: CUDA event pairs of each replica refresh are appended to timing["refresh"]
 
     def _mgpu(self):
         if self._handle is None:
@@ -197,18 +204,43 @@ class _ShardedRender(torch.nn.Module):
         except Exception:
             pass
 
+    def _refresh(self, replica, want_fine):
+        """Bring `replica` up to the primary's weights and scene (no-op when neither changed)."""
+        t = self.timing
+        if t is not None:
+            ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            ev[0].record(torch.cuda.current_stream(torch.device("cuda", self.gpus[0])))
+        replica.refresh(self.module.net, want_fine, send=self._send)
+        if t is not None:
+            ev[1].record(torch.cuda.current_stream(torch.device("cuda", self.gpus[0])))
+            t.setdefault("refresh", []).append(ev)
+
+    def _grad_mode_sharded(self, net, rays):
+        """Training on several GPUs needs the fused node: a PixelNeRFNet, CUDA rays, PNR_FUSED_BACKWARD unset / auto /
+        2 (its other values select single-GPU debugging paths) and no sigma noise (as NeRFRenderer.forward)."""
+        renderer = self.module.renderer
+        return (NeRFRenderer._is_pixelnerf(net) and rays.is_cuda
+                and os.environ.get("PNR_FUSED_BACKWARD", "auto") in ("auto", "2")
+                and not (renderer.training and renderer.noise_std > 0.0))
+
     def forward(self, rays, want_weights=False):
         net, renderer, simple = self.module.net, self.module.renderer, self.module.simple_output
-        if rays.shape[0] == 0 or rays.shape[1] == 0 or net._needs_autograd(rays):
-            if rays.shape[0] != 0 and rays.shape[1] != 0 and not self._warned:
-                warnings.warn(f"bind_parallel(net, {self.gpus}): gradients are required, so this call runs on cuda:"
-                              f"{self.gpus[0]} only (multi-GPU training = one process per GPU)")
+        empty = rays.shape[0] == 0 or rays.shape[1] == 0
+        grad = not empty and net._needs_autograd(rays)
+        if empty or (grad and not self._grad_mode_sharded(net, rays)):
+            if grad and not self._warned:
+                warnings.warn(f"bind_parallel(net, {self.gpus}): gradients are required and this model / setting has "
+                              f"no sharded backward (it needs a PixelNeRFNet, CUDA rays and PNR_FUSED_BACKWARD unset, "
+                              f"auto or 2), so this call runs on cuda:{self.gpus[0]} only")
                 self._warned = True
             return self.module(rays, want_weights=want_weights)
         if renderer.sched is not None and renderer.last_sched.item() > 0:     # as NeRFRenderer.forward (nerf.py:265-267)
             renderer.n_coarse = renderer.sched[1][renderer.last_sched.item() - 1]
             renderer.n_fine = renderer.sched[2][renderer.last_sched.item() - 1]
         want_weights = want_weights and not simple
+        if grad:
+            from .fused_train import sharded_render_train
+            return _wrapper_output(renderer, sharded_render_train(self, rays, want_weights), simple)
         Kc, Kf, Kfd = int(renderer.n_coarse), int(renderer.n_fine), int(renderer.n_fine_depth)
         fine = bool(renderer.using_fine) and Kf > 0
         if not fine:
@@ -255,7 +287,7 @@ class _ShardedRender(torch.nn.Module):
             model = net
             if i > 0:
                 model = self._replicas[g]
-                model.refresh(net, fine, send=self._send)
+                self._refresh(model, fine)
             with torch.cuda.device(dev):
                 scene, mc, mf, keep2 = model._scene_struct(want_fine=fine)
                 Ri = SB * Bi

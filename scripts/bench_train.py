@@ -7,6 +7,9 @@ with want_weights=True, MSE coarse + MSE fine, backward through MLPs and the enc
     python scripts/bench_train.py --mode field      # PNR_FUSED_BACKWARD=1: torch renderer, fused field fwd + pnr_field_backward
     python scripts/bench_train.py --mode torch      # PNR_FUSED_BACKWARD=0: composed-torch grad path of this package
     python scripts/bench_train.py --mode reference  # the UNMODIFIED reference (oracle/_ref), same step, same GPU
+    python scripts/bench_train.py --gpus "0 1"      # render mode through bind_parallel(net, [0, 1]): rays sharded over
+                                                    # the GPUs, gradients summed onto the first ("0 0": one GPU, two
+                                                    # shards -- the sharded path's overhead, not scaling)
 
 `--device cpu --tiny` checks the script itself (torch mode)."""
 import argparse
@@ -33,7 +36,13 @@ def main():
     ap.add_argument("--SB", type=int, default=4)
     ap.add_argument("--B", type=int, default=128)
     ap.add_argument("--tiny", action="store_true", help="d_hidden 32, 8+4 samples, 32x32 images: a script self-check")
+    ap.add_argument("--gpus", default=None, help='device ids as train.py\'s --gpu_id, e.g. "0 1" (render mode)')
     a = ap.parse_args()
+    gpus = [int(x) for x in a.gpus.split()] if a.gpus else None
+    if gpus:
+        if a.mode != "render":
+            ap.error("--gpus needs --mode render")
+        a.device = f"cuda:{gpus[0]}"
     os.environ["PNR_FUSED_BACKWARD"] = {"torch": "0", "field": "1", "render": "2", "reference": "0"}[a.mode]
     dev = torch.device(a.device)
     W = H = 128
@@ -69,7 +78,21 @@ def main():
         for mlp in (net.mlp_coarse, net.mlp_fine):
             for blk in mlp.blocks:
                 blk.fc_1.weight.normal_(0, 0.03)
-    render_par = renderer.bind_parallel(net, None).train()
+    render_par = renderer.bind_parallel(net, gpus).train()
+    sharded = hasattr(render_par, "gpus")
+    timing = {"forward": [], "backward": []}
+    if sharded:
+        render_par.timing = timing
+
+    def timed(name, fn):
+        if not (gpus and dev.type == "cuda"):
+            return fn()
+        ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev[0].record()
+        r = fn()
+        ev[1].record()
+        timing[name].append(ev)
+        return r
     opt = torch.optim.Adam(net.parameters(), lr=1e-4)
     NS, SB, B = 2, a.SB, a.B
     z_near, z_far, focal = 0.8, 1.8, torch.tensor(131.25 * W / 128.0)
@@ -89,12 +112,12 @@ def main():
     def step():
         images, src, rays, gt = batch()
         net.encode(images, src, focal.to(dev))
-        out = render_par(rays, want_weights=True)
+        out = timed("forward", lambda: render_par(rays, want_weights=True))
         loss = torch.nn.functional.mse_loss(out["coarse"]["rgb"], gt)
         if "fine" in out and len(out["fine"]) > 0:
             loss = loss + torch.nn.functional.mse_loss(out["fine"]["rgb"], gt)
         opt.zero_grad()
-        loss.backward()
+        timed("backward", loss.backward)
         opt.step()
         return float(loss.detach())
 
@@ -102,13 +125,46 @@ def main():
     for _ in range(a.warmup):
         step()
     sync()
+    for v in timing.values():
+        v.clear()
     t0 = time.perf_counter()
     losses = [step() for _ in range(a.steps)]
     sync()
     dt = time.perf_counter() - t0
-    print(json.dumps({"metric": "training rays/s (encode + render fwd/bwd + Adam)", "mode": a.mode,
-                      "value": SB * B * a.steps / dt, "ms_per_step": dt / a.steps * 1e3, "SB": SB, "B": B,
-                      "loss_first": losses[0], "loss_last": losses[-1], "finite": bool(np.isfinite(losses).all())}))
+    res = {"metric": "training rays/s (encode + render fwd/bwd + Adam)", "mode": a.mode,
+           "value": SB * B * a.steps / dt, "ms_per_step": dt / a.steps * 1e3, "SB": SB, "B": B,
+           "loss_first": losses[0], "loss_last": losses[-1], "finite": bool(np.isfinite(losses).all())}
+    if gpus:
+        # device ms per step on the first GPU's stream (forward includes the replica refresh, backward the reduction)
+        per_step = lambda evs: sum(e[0].elapsed_time(e[1]) for e in evs) / a.steps
+        res.update(gpus=gpus, gpu=torch.cuda.get_device_name(dev),
+                   forward_ms=per_step(timing["forward"]), backward_ms=per_step(timing["backward"]),
+                   refresh_ms=per_step(timing.get("refresh", [])), reduction_ms=reduction_ms(net, gpus, dev, a.steps))
+    print(json.dumps(res))
+
+
+def reduction_ms(net, gpus, dev, reps):
+    """Device ms of the backward's reduction at this shape, timed on its own: pnr_sum_into of len(gpus) - 1 gradient
+    arenas (both MLPs' parameter gradients + the channels-last latent gradient) into device 0's.  Where device 0
+    cannot read a shard's device (e.g. "0 0"), the step also copies that arena to device 0 first; that copy is not
+    in this number."""
+    import ctypes as C
+    import pnr_native as pn
+    if len(gpus) < 2:
+        return 0.0
+    count = sum(p.numel() for m in (net.mlp_coarse, net.mlp_fine) for p in m.parameters()) + net.encoder.latent.numel()
+    dst = torch.zeros(count, device=dev)
+    srcs = [torch.ones(count, device=torch.device("cuda", g)) for g in gpus[1:]]
+    ptrs = (C.c_void_p * len(srcs))(*[t.data_ptr() for t in srcs])
+    torch.cuda.synchronize()
+    ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    with torch.cuda.device(dev):
+        ev[0].record()
+        for _ in range(reps):
+            pn.check(pn.lib().pnr_sum_into(C.c_void_p(dst.data_ptr()), ptrs, len(srcs), count, pn.stream_ptr(dev)))
+        ev[1].record()
+    torch.cuda.synchronize()
+    return ev[0].elapsed_time(ev[1]) / reps
 
 
 if __name__ == "__main__":

@@ -131,6 +131,16 @@ typedef struct PnrRenderGrad {
   const float* d_weights_fine;   /* [R][Kc+Kf]  */
 } PnrRenderGrad;
 
+/* Gradients w.r.t. the source cameras that PixelNeRFNet.encode leaves in PnrScene (models.py:112-141), for a loss on
+ * what the field / renderer computed from them (models.py:161-212).  Each is accumulated (+=); any pointer may be NULL
+ * (not wanted).  The world->camera poses' gradient reaches encode()'s camera->world poses through the caller's
+ * autograd (rot = R^T, t = -R^T T). */
+typedef struct PnrCameraGrad {
+  float* d_poses;  /* [V][3][4] as PnrScene.poses          */
+  float* d_focal;  /* [n_focal][2] as PnrScene.focal (fx, -fy) */
+  float* d_c;      /* [n_c][2] as PnrScene.c                */
+} PnrCameraGrad;
+
 int pnr_abi_version(void);
 const char* pnr_last_error(void);
 
@@ -150,6 +160,17 @@ int pnr_sample_coarse(const float* rays, const float* lin_steps, const float* u_
 int pnr_gen_rays(const float* poses_c2w, int64_t NV, int32_t W, int32_t H, float fx, float fy, float cx,
                  float cy, float z_near, float z_far, int64_t first, int64_t count, float* rays,
                  void* stream);
+
+/* Backward of pnr_gen_rays w.r.t. the poses (util.py:251-254: origins = poses[:, :3, 3], dirs = poses[:, :3, :3]
+ * unproj): d_rays [count][8] of pixels [first, first+count) -> d_poses_c2w [NV][4][4], accumulated (+=):
+ * d_t += sum_pixels d_origin, d_R += sum_pixels d_dir unproj^T.  Rows 3 and the near / far columns get nothing (near
+ * and far are constants there).  Each pose's pixels are summed by one block in a fixed order (no atomics), so repeated
+ * calls give the same bits; one block per camera means a single large view is summed by one SM (not the training
+ * path's cost: a training step's rays are a few thousand pixels).  Intrinsics are host floats, as in pnr_gen_rays: not
+ * differentiated. */
+int pnr_gen_rays_backward(const float* d_rays, const float* poses_c2w, int64_t NV, int32_t W, int32_t H, float fx,
+                          float fy, float cx, float cy, int64_t first, int64_t count, float* d_poses_c2w,
+                          void* stream);
 
 /* Frame assembly of eval/gen_video.py:213-222 + :236: out[i] = (uint8)(rgb[i] * 255), truncating
  * (numpy astype); n = number of float values (rays * 3).  Values outside [0, 256/255) wrap like the
@@ -185,6 +206,16 @@ size_t pnr_field_backward_workspace_bytes(const PnrScene* scene, const PnrMlp* m
 int pnr_field_backward(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
                        const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz, int64_t P,
                        void* workspace, size_t workspace_bytes, void* stream);
+/* pnr_field_backward plus the gradients of the view directions and the cameras (models.py:161-212):
+ *   d_viewdirs : [SB][P][3] = sum over views of R^T d(R dir) (overwritten); may be NULL
+ *   cam        : camera gradients (+=), see PnrCameraGrad; may be NULL.  With q = R x, p = q + t, uv = -p.xy/p.z f + c:
+ *                d_R += dq (x) x + d(R dir) (x) dir, d_t += d_p (projection part), d_f += d_uv * (-p.xy/p.z),
+ *                d_c += d_uv; per-(point, view) partials are reduced per view in a fixed order (no atomics).
+ * Same workspace as pnr_field_backward; with d_viewdirs and cam NULL it is pnr_field_backward. */
+int pnr_field_backward_cam(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
+                           const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz,
+                           float* d_viewdirs, const PnrCameraGrad* cam, int64_t P, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* Backward of the compositing tail (pnr_composite; oracle/pnr_aux_backward.py::composite_backward): upstream gradients
  * d_rgb [R][3], d_depth [R], d_weights [R][K] (each may be NULL = zero) ->
@@ -213,6 +244,22 @@ int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, cons
                            const PnrRenderOut* fwd, const PnrRenderGrad* up, const PnrMlp* grad_coarse,
                            const PnrMlp* grad_fine, float* d_latent_nhwc, int64_t B, void* workspace,
                            size_t workspace_bytes, void* stream);
+
+/* pnr_render_backward_ex plus the gradients of the rays and the source cameras (nerf.py:98-204, models.py:161-212):
+ *   d_rays : [SB][B][8] = d(origin, direction, near, far), overwritten; NULL = not wanted.  points = o + z d and
+ *            viewdirs = d (nerf.py:185, 204); the sample depths send their gradient to near / far through
+ *            z = near (1 - s) + far s (stratified and importance samples of both passes, nerf.py:111-113, 146-147), the
+ *            depth-centred samples z = max(min(depth + n std, far), near) (nerf.py:160) to the coarse depth, far or
+ *            near as torch's min / max route it, and the last interval far - z_{K-1} (nerf.py:181) to far.
+ *   cam    : camera gradients of both passes (+=), see PnrCameraGrad and pnr_field_backward_cam; NULL = none.
+ * With both NULL this is pnr_render_backward_ex (same kernels, same bits); otherwise the coarse pass's positions
+ * gradient is computed as well.  Not differentiated: image_shape and latent_scaling (buffers, as in the reference).
+ * Same workspace as pnr_render_backward_ex. */
+int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                            const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise,
+                            const PnrRenderOut* fwd, const PnrRenderGrad* up, const PnrMlp* grad_coarse,
+                            const PnrMlp* grad_fine, float* d_latent_nhwc, float* d_rays, const PnrCameraGrad* cam,
+                            int64_t B, void* workspace, size_t workspace_bytes, void* stream);
 
 /* pnr_render_backward_ex for a loss on the two rgb outputs only (train/train.py:199-215: MSE coarse + MSE fine):
  *   d_rgb_*      : [SB*B][3] upstream gradients, required (d_rgb_fine NULL when n_fine == 0)
@@ -291,6 +338,14 @@ typedef struct PnrShardGrad {     /* everything device i needs for its piece of 
   void* stream;                   /* stream on device i (NULL: the handle's own stream)                               */
 } PnrShardGrad;
 
+/* Ray and camera gradients of a sharded step (pnr_render_backward_cam on every shard): one per shard, on device i. */
+typedef struct PnrShardCam {
+  PnrCameraGrad cam;              /* shards i > 0: buffers inside the shard's `arena`, at the offsets cam0 has in device */
+                                  /*   0's arena, so the reduction sums them in shard order (shard 0: cam0 is used)      */
+  float* d_rays;                  /* [SB][B_i][8] staging on device i, copied into rows [a, b) of d_rays0 (unused for   */
+                                  /*   shard 0 of one object, which writes d_rays0 in place)                            */
+} PnrShardCam;
+
 int pnr_mgpu_create(const int32_t* device_ids, int32_t n, PnrMgpu** out);   /* enables peer access towards device_ids[0] */
 int pnr_mgpu_destroy(PnrMgpu* h);
 int32_t pnr_mgpu_size(const PnrMgpu* h);
@@ -309,6 +364,17 @@ int pnr_mgpu_render(PnrMgpu* h, const PnrShard* shards, const PnrRenderCfg* cfg,
 int pnr_mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
                              const PnrRenderCfg* cfg, const PnrRenderGrad* up0, const PnrMlp* grad_coarse0,
                              const PnrMlp* grad_fine0, float* d_latent0_nhwc, int64_t B, void* stream0);
+/* pnr_mgpu_render_backward plus the gradients of the rays and the source cameras (pnr_render_backward_cam):
+ *   d_rays0     : [SB][B][8] on device 0, overwritten; NULL = not wanted.  Each shard's rows come back as the reverse
+ *                 of the forward's strided ray staging.
+ *   cam0        : device 0's camera gradients (+=), inside shard 0's arena when there are several shards; NULL = none.
+ *   shard_cams  : [n] per-shard buffers (PnrShardCam); may be NULL when d_rays0 and cam0 are.
+ * Camera gradients of every shard are summed onto cam0 by the same reduction as the weights, in shard order.  With
+ * d_rays0 and cam0 NULL this is pnr_mgpu_render_backward. */
+int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
+                                 const PnrShardCam* shard_cams, const PnrRenderCfg* cfg, const PnrRenderGrad* up0,
+                                 const PnrMlp* grad_coarse0, const PnrMlp* grad_fine0, float* d_latent0_nhwc,
+                                 float* d_rays0, const PnrCameraGrad* cam0, int64_t B, void* stream0);
 /* The reduction step on its own: dst[j] += src[0][j] + src[1][j] + ... + src[n-1][j], added left to right, for
  * j < count.  src: host array of n <= 63 device pointers readable from the current device. */
 int pnr_sum_into(float* dst, const float* const* src, int32_t n, int64_t count, void* stream);

@@ -170,6 +170,17 @@ int pnr_gen_rays(const float* poses_c2w, int64_t NV, int32_t W, int32_t H, float
   return launch_gen_rays(poses_c2w, W, H, fx, fy, cx, cy, z_near, z_far, first, count, rays, (cudaStream_t)stream);
 }
 
+int pnr_gen_rays_backward(const float* d_rays, const float* poses_c2w, int64_t NV, int32_t W, int32_t H, float fx,
+                          float fy, float cx, float cy, int64_t first, int64_t count, float* d_poses_c2w,
+                          void* stream) {
+  PNR_CHECK_ARG(NV >= 0 && W >= 1 && H >= 1, "bad sizes");
+  PNR_CHECK_ARG(first >= 0 && count >= 0 && first + count <= NV * (int64_t)W * H, "ray range outside the pixel grid");
+  if (count == 0) return PNR_OK;
+  PNR_CHECK_ARG(d_rays && poses_c2w && d_poses_c2w, "NULL pointer");
+  PNR_CHECK_ARG(fx != 0.f && fy != 0.f, "zero focal length");
+  return launch_gen_rays_bwd(d_rays, W, H, fx, fy, cx, cy, first, count, d_poses_c2w, (cudaStream_t)stream);
+}
+
 int pnr_frames_u8(const float* rgb, int64_t n, uint8_t* out, void* stream) {
   PNR_CHECK_ARG(n >= 0, "bad size");
   if (n == 0) return PNR_OK;
@@ -245,6 +256,14 @@ size_t pnr_field_backward_workspace_bytes(const PnrScene* scene, const PnrMlp* m
 int pnr_field_backward(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
                        const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz, int64_t P,
                        void* workspace, size_t workspace_bytes, void* stream) {
+  return pnr_field_backward_cam(scene, mlp, xyz, viewdirs, d_out, grad, d_latent_nhwc, d_xyz, nullptr, nullptr, P,
+                                workspace, workspace_bytes, stream);
+}
+
+int pnr_field_backward_cam(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
+                           const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz,
+                           float* d_viewdirs, const PnrCameraGrad* cam, int64_t P, void* workspace,
+                           size_t workspace_bytes, void* stream) {
   int rc;
   if ((rc = check_scene(scene))) return rc;
   if ((rc = check_mlp(mlp))) return rc;
@@ -261,8 +280,8 @@ int pnr_field_backward(const PnrScene* scene, const PnrMlp* mlp, const float* xy
   src.dirs = viewdirs;
   src.P = P;
   src.K = 1;
-  return field_backward(*scene, *mlp, src, P * scene->SB, d_out, *grad, d_latent_nhwc, d_xyz, workspace,
-                        workspace_bytes, (cudaStream_t)stream);
+  return field_backward(*scene, *mlp, src, P * scene->SB, d_out, *grad, d_latent_nhwc, d_xyz, d_viewdirs, cam,
+                        workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 static size_t render_bwd_field_ws(const PnrScene& sc, const PnrMlp& m, int64_t pts) {
@@ -280,6 +299,8 @@ size_t pnr_render_backward_workspace_bytes(const PnrScene* scene, const PnrMlp* 
   b += align_up((size_t)R * K * 4, 256);           // d_z
   b += align_up((size_t)R * K * 3 * 4, 256);       // d_xyz
   b += align_up((size_t)R * 4, 256);               // d_depth
+  b += align_up((size_t)R * K * 3 * 4, 256);       // d_vd (ray / camera gradients only)
+  b += align_up((size_t)R * 4, 256);               // d_far of the last interval (ray gradients only)
   size_t f = render_bwd_field_ws(*scene, *mlp_coarse, R * K);
   if (mlp_fine) {
     size_t f2 = render_bwd_field_ws(*scene, *mlp_fine, R * K);
@@ -310,6 +331,15 @@ int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, cons
                            const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise, const PnrRenderOut* fwd,
                            const PnrRenderGrad* up, const PnrMlp* grad_coarse, const PnrMlp* grad_fine,
                            float* d_latent_nhwc, int64_t B, void* workspace, size_t workspace_bytes, void* stream) {
+  return pnr_render_backward_cam(scene, mlp_coarse, mlp_fine, cfg, rays, noise, fwd, up, grad_coarse, grad_fine,
+                                 d_latent_nhwc, nullptr, nullptr, B, workspace, workspace_bytes, stream);
+}
+
+int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                            const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise, const PnrRenderOut* fwd,
+                            const PnrRenderGrad* up, const PnrMlp* grad_coarse, const PnrMlp* grad_fine,
+                            float* d_latent_nhwc, float* d_rays, const PnrCameraGrad* cam, int64_t B, void* workspace,
+                            size_t workspace_bytes, void* stream) {
   int rc;
   if ((rc = check_render_backward(scene, mlp_coarse, mlp_fine, cfg, noise, fwd, grad_coarse, grad_fine, B))) return rc;
   const int64_t R = B * scene->SB;
@@ -335,6 +365,13 @@ int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, cons
   float* d_z = ar.take<float>((size_t)R * K);
   float* d_xyz = ar.take<float>((size_t)R * K * 3);
   float* d_depth = ar.take<float>((size_t)R);
+  float* d_vd = ar.take<float>((size_t)R * K * 3);
+  float* d_far = ar.take<float>((size_t)R);
+  const bool want_cam = cam && (cam->d_poses || cam->d_focal || cam->d_c);
+  const bool want_rays = d_rays != nullptr;
+  if (!want_cam) cam = nullptr;
+  float* vd = want_rays ? d_vd : nullptr;
+  float* dfar = want_rays ? d_far : nullptr;
   char* rest = ar.base + align_up(ar.off, 256);
   const size_t rest_bytes = workspace_bytes - align_up(ar.off, 256);
   const float* d_depth_coarse = g.d_depth_coarse;
@@ -350,10 +387,10 @@ int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, cons
     const float* pj = mlp_fine ? scene->proj_fine : scene->proj_coarse;
     if ((rc = field_dispatch(*scene, *m, pj, src, R * K, field, cfg->engine, rest, rest_bytes, s))) return rc;
     if ((rc = launch_composite_bwd(rays, fwd->z_fine, field, g.d_rgb_fine, g.d_depth_fine, g.d_weights_fine,
-                                   cfg->white_bkgd, d_field, d_z, R, K, s)))
+                                   cfg->white_bkgd, d_field, d_z, dfar, R, K, s)))
       return rc;
-    if ((rc = field_backward(*scene, *m, src, R * K, d_field, *gm, d_latent_nhwc, depth_path ? d_xyz : nullptr, rest,
-                             rest_bytes, s)))
+    if ((rc = field_backward(*scene, *m, src, R * K, d_field, *gm, d_latent_nhwc,
+                             (depth_path || want_rays) ? d_xyz : nullptr, vd, cam, rest, rest_bytes, s)))
       return rc;
     if (depth_path) {
       if ((rc = launch_depth_grad(rays, fwd->z_fine, fwd->depth_coarse, noise->n_depth, cfg->depth_std, d_z, d_xyz,
@@ -361,17 +398,28 @@ int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, cons
         return rc;
       d_depth_coarse = d_depth;
     }
+    if (want_rays && (rc = launch_ray_grad(rays, fwd->z_fine, d_z, d_xyz, d_vd, d_far, depth_path, fwd->depth_coarse,
+                                           noise->n_depth, cfg->depth_std, Kfd, false, d_rays, R, K, s)))
+      return rc;
   }
-  if (!coarse_grad) return PNR_OK;
+  if (!coarse_grad) {
+    if (want_rays && !fine_grad) PNR_CUDA(cudaMemsetAsync(d_rays, 0, (size_t)R * 8 * sizeof(float), s));
+    return PNR_OK;
+  }
   src.z = fwd->z_coarse;
   src.K = Kc;
   src.P = B * Kc;
   if ((rc = field_dispatch(*scene, *mlp_coarse, scene->proj_coarse, src, R * Kc, field, cfg->engine, rest, rest_bytes, s)))
     return rc;
   if ((rc = launch_composite_bwd(rays, fwd->z_coarse, field, g.d_rgb_coarse, d_depth_coarse, g.d_weights_coarse,
-                                 cfg->white_bkgd, d_field, d_z, R, Kc, s)))
+                                 cfg->white_bkgd, d_field, d_z, dfar, R, Kc, s)))
     return rc;
-  return field_backward(*scene, *mlp_coarse, src, R * Kc, d_field, *grad_coarse, d_latent_nhwc, nullptr, rest, rest_bytes, s);
+  if ((rc = field_backward(*scene, *mlp_coarse, src, R * Kc, d_field, *grad_coarse, d_latent_nhwc,
+                           want_rays ? d_xyz : nullptr, vd, cam, rest, rest_bytes, s)))
+    return rc;
+  if (!want_rays) return PNR_OK;
+  return launch_ray_grad(rays, fwd->z_coarse, d_z, d_xyz, d_vd, d_far, false, nullptr, nullptr, 0.f, 0, fine_grad,
+                         d_rays, R, Kc, s);
 }
 
 int pnr_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
@@ -397,7 +445,7 @@ int pnr_composite_backward(const float* rays, const float* z, const float* field
   PNR_CHECK_ARG(R >= 0 && K >= 1, "bad sizes");
   if (R == 0) return PNR_OK;
   PNR_CHECK_ARG(rays && z && field && d_field && d_z, "NULL pointer");
-  return launch_composite_bwd(rays, z, field, d_rgb, d_depth, d_weights, white_bkgd, d_field, d_z, R, K,
+  return launch_composite_bwd(rays, z, field, d_rgb, d_depth, d_weights, white_bkgd, d_field, d_z, nullptr, R, K,
                               (cudaStream_t)stream);
 }
 

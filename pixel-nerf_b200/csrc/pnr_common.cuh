@@ -102,16 +102,24 @@ int simt_field_eval(const PnrScene& sc, const PnrMlp& mlp, const PointSource& sr
 // d_rgb [R][3], d_depth [R], d_weights [R][K], d_depth_up [R] may each be NULL (zero).
 int launch_composite_bwd(const float* rays, const float* z, const float* field, const float* d_rgb,
                          const float* d_depth, const float* d_weights, int white, float* d_field, float* d_z,
-                         int64_t R, int K, cudaStream_t s);
+                         float* d_far, int64_t R, int K, cudaStream_t s);   // d_far [R]: d(last interval), may be NULL
 int launch_depth_grad(const float* rays, const float* z_sorted, const float* depth, const float* nd,
                       float depth_std, float* d_z, const float* d_xyz, const float* d_depth_up, float* d_depth,
                       int64_t R, int K, int Kfd, cudaStream_t s);
+// ray gradient of one pass from its per-sample d_z / d_xyz / d_vd (written, or added when accum); Kfd > 0: the pass
+// holds the depth-centred samples of depth / nd (the fine pass)
+int launch_ray_grad(const float* rays, const float* z, const float* d_z, const float* d_xyz, const float* d_vd,
+                    const float* d_far_last, bool dz_has_pos, const float* depth, const float* nd, float depth_std,
+                    int Kfd, bool accum, float* d_rays, int64_t R, int K, cudaStream_t s);
+// backward of launch_gen_rays: d_rays [count][8] -> d_poses [NV][4][4] (+=)
+int launch_gen_rays_bwd(const float* d_rays, int W, int H, float fx, float fy, float cx, float cy, int64_t first,
+                        int64_t count, float* d_poses, cudaStream_t s);
 
 // ---- field backward, SIMT first path (pnr_field_bwd.cu) --------------------------------
 size_t field_backward_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int64_t total_points);
 int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src, int64_t total_points,
-                   const float* d_out, const PnrMlp& grad, float* d_latent, float* d_xyz, void* ws, size_t ws_bytes,
-                   cudaStream_t s);
+                   const float* d_out, const PnrMlp& grad, float* d_latent, float* d_xyz, float* d_dirs,
+                   const PnrCameraGrad* cam, void* ws, size_t ws_bytes, cudaStream_t s);
 
 // ---- tensor engine (pnr_field_tc.cu) ---------------------------------------------------
 bool tc_supported(const PnrScene& sc, const PnrMlp& mlp);

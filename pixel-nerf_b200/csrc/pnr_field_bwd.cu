@@ -167,8 +167,12 @@ __global__ void k_lin_out_bwd(const float* __restrict__ H, const float* __restri
 // Geometry backward, one warp per point over its NS views (rows lp*NS + v of the chunk):
 //   d_lat row (C) -> atomic scatter into d_latent (channels-last) over the 4 taps, and d(ix, iy)
 //   d_feat row (48) -> pos-enc derivative; projection; rotate back; sum over views -> d_xyz[point]
+//   optional: d_dirs[point] = sum over views of R^T d(R dir) (models.py:188-193), and per row the 16 camera partials
+//   cam_part[row] = [dR (3x3) | dt (3) in the [3][4] pose layout | d_focal (2) | d_c (2)] (models.py:161-212), which
+//   k_cam_reduce sums per view in a fixed order (no same-address atomics)
 __global__ void k_geom_bwd(PnrScene sc, PointSource src, int64_t g0, int64_t n_pts, const float* __restrict__ d_feat,
-                           const float* __restrict__ d_lat, float* __restrict__ d_latent, float* __restrict__ d_xyz) {
+                           const float* __restrict__ d_lat, float* __restrict__ d_latent, float* __restrict__ d_xyz,
+                           float* __restrict__ d_dirs, float* __restrict__ cam_part) {
   const int64_t lp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;
   const int lane = threadIdx.x % 32;
   if (lp >= n_pts) return;
@@ -176,7 +180,7 @@ __global__ void k_geom_bwd(PnrScene sc, PointSource src, int64_t g0, int64_t n_p
   const int sb = (int)(g / src.P);
   float x[3], dir[3];
   load_point(src, g, x, dir);
-  float dx[3] = {0.f, 0.f, 0.f};
+  float dx[3] = {0.f, 0.f, 0.f}, dd[3] = {0.f, 0.f, 0.f};
   const int C = sc.C, Wl = sc.Wl, Hl = sc.Hl;
   for (int v = 0; v < sc.NS; ++v) {
     const int64_t row = lp * sc.NS + v;
@@ -252,15 +256,82 @@ __global__ void k_geom_bwd(PnrScene sc, PointSource src, int64_t g0, int64_t n_p
     }
     // projection (models.py:206-212): uv = -p.xy / p.z * focal + c
     const float gz0 = d_u * fo[0], gz1 = d_w * fo[1];
-    dq[0] += -gz0 / p[2];
-    dq[1] += -gz1 / p[2];
-    dq[2] += (gz0 * p[0] + gz1 * p[1]) / (p[2] * p[2]);
+    const float dp[3] = {-gz0 / p[2], -gz1 / p[2], (gz0 * p[0] + gz1 * p[1]) / (p[2] * p[2])};
+    dq[0] += dp[0];
+    dq[1] += dp[1];
+    dq[2] += dp[2];
     for (int i = 0; i < 3; ++i) dx[i] += M[0 * 4 + i] * dq[0] + M[1 * 4 + i] * dq[1] + M[2 * 4 + i] * dq[2];   // R^T dq
+    const float* dv = df + 39;                                                     // d(R dir)
+    if (d_dirs)
+      for (int i = 0; i < 3; ++i) dd[i] += M[0 * 4 + i] * dv[0] + M[1 * 4 + i] * dv[1] + M[2 * 4 + i] * dv[2];
+    if (cam_part && lane == 0) {   // q = R x, p = q + t, dir_cam = R dir, uv = -p.xy / p.z * focal + c
+      float* cp = cam_part + row * 16;
+      for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) cp[i * 4 + j] = dq[i] * x[j] + dv[i] * dir[j];
+        cp[i * 4 + 3] = dp[i];
+      }
+      cp[12] = d_u * (-p[0] / p[2]);
+      cp[13] = d_w * (-p[1] / p[2]);
+      cp[14] = d_u;
+      cp[15] = d_w;
+    }
   }
   if (d_xyz && lane == 0) {
     d_xyz[g * 3 + 0] = dx[0];
     d_xyz[g * 3 + 1] = dx[1];
     d_xyz[g * 3 + 2] = dx[2];
+  }
+  if (d_dirs && lane == 0) {
+    d_dirs[g * 3 + 0] = dd[0];
+    d_dirs[g * 3 + 1] = dd[1];
+    d_dirs[g * 3 + 2] = dd[2];
+  }
+}
+
+// Camera partials of one chunk, summed per source view: block vi = sb*NS + v adds, over the chunk's points of object
+// sb in a fixed order (thread-strided partial sums, then a shared-memory tree), its 16 partials into acc[vi][16].
+// One writer per address and chunks in stream order, so the result does not depend on scheduling.
+constexpr int kCamThreads = 256;
+__global__ void __launch_bounds__(kCamThreads) k_cam_reduce(const float* __restrict__ cam_part, int64_t g0,
+                                                            int64_t n_pts, int64_t P, int NS, float* __restrict__ acc) {
+  __shared__ float red[16][kCamThreads];
+  const int vi = blockIdx.x, sb = vi / NS, v = vi - sb * NS, t = threadIdx.x;
+  int64_t a = (int64_t)sb * P - g0, b = (int64_t)(sb + 1) * P - g0;   // local points of object sb
+  if (a < 0) a = 0;
+  if (b > n_pts) b = n_pts;
+  float s[16];
+  for (int j = 0; j < 16; ++j) s[j] = 0.f;
+  for (int64_t lp = a + t; lp < b; lp += kCamThreads) {
+    const float* cp = cam_part + (lp * NS + v) * 16;
+    for (int j = 0; j < 16; ++j) s[j] += cp[j];
+  }
+  for (int j = 0; j < 16; ++j) red[j][t] = s[j];
+  __syncthreads();
+  for (int w = kCamThreads / 2; w > 0; w >>= 1) {
+    if (t < w)
+      for (int j = 0; j < 16; ++j) red[j][t] += red[j][t + w];
+    __syncthreads();
+  }
+  if (t < 16 && b > a) acc[vi * 16 + t] += red[t][0];
+}
+
+// acc [V][16] -> d_poses [V][3][4] (+=), d_focal [n_focal][2] (+=) and d_c [n_c][2] (+=); a shared focal / c row sums
+// the views of every object, in view order.
+__global__ void k_cam_finish(const float* __restrict__ acc, int V, int NS, int n_focal, int n_c,
+                             float* __restrict__ d_poses, float* __restrict__ d_focal, float* __restrict__ d_c) {
+  const int t = threadIdx.x;
+  if (d_poses)
+    for (int i = t; i < V * 12; i += blockDim.x) d_poses[i] += acc[(i / 12) * 16 + i % 12];
+  if (t < 4) {
+    float* dst = t < 2 ? d_focal : d_c;
+    const int rows = t < 2 ? n_focal : n_c, k = t & 1, col = 12 + t;
+    if (dst)
+      for (int r = 0; r < rows; ++r) {
+        const int v0 = rows > 1 ? r * NS : 0, v1 = rows > 1 ? (r + 1) * NS : V;
+        float sum = 0.f;
+        for (int vi = v0; vi < v1; ++vi) sum += acc[vi * 16 + col];
+        dst[r * 2 + k] += sum;
+      }
   }
 }
 
@@ -277,7 +348,8 @@ static int64_t chunk_points(const PnrScene& sc, int64_t total_points) {
 
 struct Bufs {
   float *feat, *lat, *latT, *featT, *hpre[PNR_MAX_BLOCKS], *nbuf[PNR_MAX_BLOCKS], *xv, *hlast, *dh, *dhv, *T, *T2, *tA, *tB,
-      *dlat, *dfeat, *do4, *w_in, *w_inT, *tmp_win, *w0T[PNR_MAX_BLOCKS], *w1T[PNR_MAX_BLOCKS], *wzT[PNR_MAX_BLOCKS];
+      *dlat, *dfeat, *do4, *w_in, *w_inT, *tmp_win, *w0T[PNR_MAX_BLOCKS], *w1T[PNR_MAX_BLOCKS], *wzT[PNR_MAX_BLOCKS],
+      *cam_acc;
 };
 
 static size_t carve(Arena& ar, Bufs& b, const PnrScene& sc, const PnrMlp& mlp, int64_t cp) {
@@ -307,6 +379,7 @@ static size_t carve(Arena& ar, Bufs& b, const PnrScene& sc, const PnrMlp& mlp, i
   b.w_in = ar.take<float>(d * 48);
   b.w_inT = ar.take<float>(48 * d);
   b.tmp_win = ar.take<float>(d * 48);
+  b.cam_acc = ar.take<float>((size_t)sc.SB * sc.NS * 16);
   return ar.off;
 }
 
@@ -325,8 +398,8 @@ size_t field_backward_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int
   } while (0)
 
 int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src, int64_t total_points,
-                   const float* d_out, const PnrMlp& grad, float* d_latent, float* d_xyz, void* ws, size_t ws_bytes,
-                   cudaStream_t s) {
+                   const float* d_out, const PnrMlp& grad, float* d_latent, float* d_xyz, float* d_dirs,
+                   const PnrCameraGrad* cam, void* ws, size_t ws_bytes, cudaStream_t s) {
   using namespace bwd;
   PNR_CHECK_ARG(mlp.d_in == 42 && mlp.d_out == 4, "backward expects d_in == 42, d_out == 4");
   PNR_CHECK_ARG(mlp.d_hidden % 16 == 0 && mlp.d_latent % 16 == 0, "d_hidden and d_latent must be multiples of 16");
@@ -346,6 +419,9 @@ int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src
   Arena ar(ws, ws_bytes);
   Bufs b;
   carve(ar, b, sc, mlp, cp);
+  const bool want_cam = cam && (cam->d_poses || cam->d_focal || cam->d_c);
+  const int V = sc.SB * NS;
+  if (want_cam) PNR_CUDA(cudaMemsetAsync(b.cam_acc, 0, (size_t)V * 16 * sizeof(float), s));
 
   // transposed weights, once per call: W [out][in] -> W^T [in][out]
   k_pad_rows<<<(d * 48 + 255) / 256, 256, 0, s>>>(mlp.lin_in_w, b.w_in, d, mlp.d_in, 48);
@@ -452,7 +528,17 @@ int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src
     PNR_LAUNCH_CHECK();
     BW(rowsum_acc(b.tA, Rp, d, const_cast<float*>(grad.lin_in_b), s));
     BW(gemm(dh, d, b.w_inT, nullptr, b.dfeat, 48, R, 48, d, false, false, s));
-    k_geom_bwd<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(sc, src, g0, n, b.dfeat, b.dlat, d_latent, d_xyz);
+    float* cam_part = want_cam ? b.T : nullptr;    // [R][16]; T (R x d, d >= 16) is free again here
+    k_geom_bwd<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(sc, src, g0, n, b.dfeat, b.dlat, d_latent, d_xyz,
+                                                               d_dirs, cam_part);
+    PNR_LAUNCH_CHECK();
+    if (want_cam) {
+      k_cam_reduce<<<V, kCamThreads, 0, s>>>(cam_part, g0, n, src.P, NS, b.cam_acc);
+      PNR_LAUNCH_CHECK();
+    }
+  }
+  if (want_cam) {
+    k_cam_finish<<<1, 256, 0, s>>>(b.cam_acc, V, NS, sc.n_focal, sc.n_c, cam->d_poses, cam->d_focal, cam->d_c);
     PNR_LAUNCH_CHECK();
   }
   return PNR_OK;

@@ -321,7 +321,26 @@ int pnr_sum_into(float* dst, const float* const* src, int32_t n, int64_t count, 
 int pnr_mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
                              const PnrRenderCfg* cfg, const PnrRenderGrad* up0, const PnrMlp* grad_coarse0,
                              const PnrMlp* grad_fine0, float* d_latent0_nhwc, int64_t B, void* stream0) {
+  return pnr_mgpu_render_backward_cam(h, shards, shard_grads, nullptr, cfg, up0, grad_coarse0, grad_fine0,
+                                      d_latent0_nhwc, nullptr, nullptr, B, stream0);
+}
+
+int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
+                                 const PnrShardCam* shard_cams, const PnrRenderCfg* cfg, const PnrRenderGrad* up0,
+                                 const PnrMlp* grad_coarse0, const PnrMlp* grad_fine0, float* d_latent0_nhwc,
+                                 float* d_rays0, const PnrCameraGrad* cam0, int64_t B, void* stream0) {
   PNR_CHECK_ARG(h && shards && shard_grads && cfg && grad_coarse0, "NULL argument");
+  const PnrCameraGrad c0 = cam0 ? *cam0 : PnrCameraGrad{};
+  const bool want_cam = c0.d_poses || c0.d_focal || c0.d_c;
+  // shard i's camera buffers: those of cam0 that are wanted, at the same arena offsets on device i
+  auto shard_cam = [&](int i) {
+    if (i == 0) return c0;
+    PnrCameraGrad ci = shard_cams[i].cam;
+    if (!c0.d_poses) ci.d_poses = nullptr;
+    if (!c0.d_focal) ci.d_focal = nullptr;
+    if (!c0.d_c) ci.d_c = nullptr;
+    return ci;
+  };
   PNR_CHECK_ARG(B >= 0, "B must be >= 0");
   PNR_CHECK_ARG(cfg->n_coarse >= 1 && cfg->n_fine >= 0, "bad sample counts");
   DevGuard guard;
@@ -361,7 +380,17 @@ int pnr_mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardG
                         same_offset(sg.d_latent_nhwc, sg.arena, d_latent0_nhwc, sg0.arena, sg0.arena_count),
                     "shard gradient arena must have device 0's layout");
       PNR_CHECK_ARG(h->peer_from_0[i] || sg.arena_stage0, "shard gradient needs a device-0 staging arena (no peer access)");
+      if (want_cam) {
+        PNR_CHECK_ARG(shard_cams, "camera gradients need the per-shard camera buffers");
+        const PnrCameraGrad ci = shard_cam(i);
+        PNR_CHECK_ARG(same_offset(ci.d_poses, sg.arena, c0.d_poses, sg0.arena, sg0.arena_count) &&
+                          same_offset(ci.d_focal, sg.arena, c0.d_focal, sg0.arena, sg0.arena_count) &&
+                          same_offset(ci.d_c, sg.arena, c0.d_c, sg0.arena, sg0.arena_count),
+                      "shard camera gradients must sit in the arena at device 0's offsets");
+      }
     }
+    if (d_rays0 && (i > 0 || SB > 1))
+      PNR_CHECK_ARG(shard_cams && shard_cams[i].d_rays, "ray gradients need a per-shard staging buffer");
     used = i + 1;
   }
   if (used == 0) return PNR_OK;
@@ -401,10 +430,17 @@ int pnr_mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardG
     fwd.z_coarse = const_cast<float*>(sg.z_coarse);
     fwd.z_fine = const_cast<float*>(sg.z_fine);
     fwd.depth_coarse = const_cast<float*>(sg.depth_coarse);
-    int rc = pnr_render_backward_ex(sh.scene, sh.mlp_coarse, sh.mlp_fine, cfg, sg.rays, sh.noise, &fwd, &gi,
-                                    i == 0 ? grad_coarse0 : sg.grad_coarse, i == 0 ? grad_fine0 : sg.grad_fine,
-                                    i == 0 ? d_latent0_nhwc : sg.d_latent_nhwc, Bi, sg.workspace, sg.workspace_bytes, s);
+    // ray gradients: shard 0 of one object writes device 0's rows in place, the others a staging buffer
+    const bool in_place = i == 0 && SB == 1;
+    float* dr = d_rays0 ? (in_place ? d_rays0 : shard_cams[i].d_rays) : nullptr;
+    const PnrCameraGrad ci = want_cam ? shard_cam(i) : PnrCameraGrad{};
+    int rc = pnr_render_backward_cam(sh.scene, sh.mlp_coarse, sh.mlp_fine, cfg, sg.rays, sh.noise, &fwd, &gi,
+                                     i == 0 ? grad_coarse0 : sg.grad_coarse, i == 0 ? grad_fine0 : sg.grad_fine,
+                                     i == 0 ? d_latent0_nhwc : sg.d_latent_nhwc, dr, want_cam ? &ci : nullptr, Bi,
+                                     sg.workspace, sg.workspace_bytes, s);
     if (rc) return rc;
+    // the reverse of the forward's ray staging: [SB][B_i][8] -> rows [a, b) of each object in d_rays0 [SB][B][8]
+    if (dr && !in_place && (rc = copy_rows(d_rays0 + a * 8, B * 8, dr, Bi * 8, Bi * 8, SB, s))) return rc;
     if (i > 0) PNR_CUDA(cudaEventRecord(h->done[i], s));
   }
   // device 0: grad0 += g_1 + ... + g_{used-1}, one launch over the arenas, shards in order

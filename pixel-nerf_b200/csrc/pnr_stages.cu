@@ -252,7 +252,8 @@ int launch_frames_u8(const float* rgb, int64_t n, uint8_t* out, cudaStream_t s) 
 __global__ void k_composite_bwd(const float* __restrict__ rays, const float* __restrict__ z,
                                 const float* __restrict__ field, const float* __restrict__ d_rgb,
                                 const float* __restrict__ d_depth, const float* __restrict__ d_weights, int white,
-                                float* __restrict__ d_field, float* __restrict__ d_z, int64_t R, int K) {
+                                float* __restrict__ d_field, float* __restrict__ d_z, float* __restrict__ d_far,
+                                int64_t R, int K) {
   int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= R) return;
   const float far = rays[r * 8 + 7];
@@ -302,14 +303,15 @@ __global__ void k_composite_bwd(const float* __restrict__ rays, const float* __r
     T = T * t;
     zk = znext;
   }
+  if (d_far) d_far[r] = carry;                        // delta_{K-1} = far - z_{K-1} (nerf.py:181): d_far += d_delta
 }
 
 int launch_composite_bwd(const float* rays, const float* z, const float* field, const float* d_rgb,
                          const float* d_depth, const float* d_weights, int white, float* d_field, float* d_z,
-                         int64_t R, int K, cudaStream_t s) {
+                         float* d_far, int64_t R, int K, cudaStream_t s) {
   if (R == 0) return PNR_OK;
   k_composite_bwd<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(rays, z, field, d_rgb, d_depth, d_weights, white,
-                                                              d_field, d_z, R, K);
+                                                              d_field, d_z, d_far, R, K);
   PNR_LAUNCH_CHECK();
   return PNR_OK;
 }
@@ -321,6 +323,26 @@ __global__ void k_dz_from_dxyz(float* __restrict__ d_z, const float* __restrict_
   if (i >= R * K) return;
   const float* rr = rays + (i / K) * 8;
   d_z[i] += (d_xyz[i * 3 + 0] * rr[3] + d_xyz[i * 3 + 1] * rr[4]) + d_xyz[i * 3 + 2] * rr[5];
+}
+
+// Slot of depth sample j in the sorted merged row zs [K] (the forward's rank rule: smaller values first, ties by original
+// index, the depth samples being the last index group); v = its clamped value.  k_depth_grad and k_ray_grad both route
+// a depth sample's d_z through this one function, so they agree slot for slot.
+__device__ __forceinline__ int depth_slot(const float* zs, int K, const float* ndr, int Kfd, int j, float d, float std_,
+                                          float near, float far, float v) {
+  int lo = 0, hi = K;
+  while (lo < hi) {
+    int mid = (lo + hi) >> 1;
+    if (zs[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  int ub = lo;
+  while (ub < K && zs[ub] == v) ++ub;
+  int n_eq_depth = 0, n_eq_before = 0;
+  for (int q = 0; q < Kfd; ++q) {
+    const float zq = fmaxf(fminf(d + ndr[q] * std_, far), near);
+    if (zq == v) { ++n_eq_depth; if (q < j) ++n_eq_before; }
+  }
+  return lo + ((ub - lo) - n_eq_depth) + n_eq_before;
 }
 
 // Gradient of the coarse depth through the depth-centred fine samples (nerf.py:150-161, 289-295): each sample
@@ -340,22 +362,135 @@ __global__ void k_depth_grad(const float* __restrict__ rays, const float* __rest
     const float zz = d + nd[r * Kfd + j] * depth_std;
     if (!(zz >= near && zz <= far)) continue;            // clamped: no gradient
     const float v = fmaxf(fminf(zz, far), near);
-    int lo = 0, hi = K;                                  // lower bound: first slot with value >= v
-    while (lo < hi) {
-      int mid = (lo + hi) >> 1;
-      if (zs[mid] < v) lo = mid + 1; else hi = mid;
-    }
-    int ub = lo;
-    while (ub < K && zs[ub] == v) ++ub;
-    int n_eq_depth = 0, n_eq_before = 0;
-    for (int q = 0; q < Kfd; ++q) {
-      const float zq = fmaxf(fminf(d + nd[r * Kfd + q] * depth_std, far), near);
-      if (zq == v) { ++n_eq_depth; if (q < j) ++n_eq_before; }
-    }
-    const int pos = lo + ((ub - lo) - n_eq_depth) + n_eq_before;
+    const int pos = depth_slot(zs, K, nd + r * Kfd, Kfd, j, d, depth_std, near, far, v);
     if (pos >= 0 && pos < K) acc += d_z[r * K + pos];
   }
   d_depth[r] = d_depth_up ? d_depth_up[r] + acc : acc;
+}
+
+// Ray gradient of one pass (nerf.py:98-118, 120-161, 178-204): d_rays[r] = [d_origin, d_dir, d_near, d_far], written
+// (accum = 0) or added (accum = 1).  points = o + z d and viewdirs = d give d_o = sum_k d_x, d_d = sum_k z_k d_x + d_vd;
+// the sample depths' gradient d_z (+ d_x . d unless d_z already holds it) goes to near / far through
+// z = near (1 - s) + far s, s = (z - near) / (far - near), for the stratified and importance samples; a depth-centred
+// sample z = max(min(depth + n std, far), near) sends it to far or near when clamped (k_depth_grad carries the unclamped
+// ones to the coarse depth); the last interval far - z_{K-1} adds d_far_last.
+__global__ void k_ray_grad(const float* __restrict__ rays, const float* __restrict__ z, const float* __restrict__ d_z,
+                           const float* __restrict__ d_xyz, const float* __restrict__ d_vd,
+                           const float* __restrict__ d_far_last, int dz_has_pos, const float* __restrict__ depth,
+                           const float* __restrict__ nd, float depth_std, int Kfd, int accum,
+                           float* __restrict__ d_rays, int64_t R, int K) {
+  int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  const float* rr = rays + r * 8;
+  const float near = rr[6], far = rr[7], dir[3] = {rr[3], rr[4], rr[5]};
+  const float* zr = z + r * K;
+  const float* dzr = d_z + r * K;
+  const float* dxr = d_xyz + r * K * 3;
+  const float* dvr = d_vd + r * K * 3;
+  auto dz_total = [&](int k) {
+    const float* dx = dxr + k * 3;
+    return dz_has_pos ? dzr[k] : dzr[k] + ((dx[0] * dir[0] + dx[1] * dir[1]) + dx[2] * dir[2]);
+  };
+  uint32_t is_depth[kMaxK / 32];
+  for (int i = 0; i < kMaxK / 32; ++i) is_depth[i] = 0u;
+  float g_near = 0.f, g_far = d_far_last[r];
+  if (Kfd > 0) {
+    const float d = depth[r];
+    const float* ndr = nd + r * Kfd;
+    for (int j = 0; j < Kfd; ++j) {
+      const float zz = d + ndr[j] * depth_std;
+      const float v = fmaxf(fminf(zz, far), near);
+      const int pos = depth_slot(zr, K, ndr, Kfd, j, d, depth_std, near, far, v);
+      if (pos < 0 || pos >= K) continue;
+      is_depth[pos >> 5] |= 1u << (pos & 31);
+      // torch.min chose far / torch.max chose near; at zz == far or zz == near exactly torch splits the gradient in
+      // halves, here (as in k_depth_grad) all of it goes to the depth -- a tie of measure zero
+      if (zz > far) g_far += dz_total(pos);
+      else if (zz < near) g_near += dz_total(pos);
+    }
+  }
+  float go[3] = {0.f, 0.f, 0.f}, gd[3] = {0.f, 0.f, 0.f};
+  const float span = far - near;
+  for (int k = 0; k < K; ++k) {
+    const float* dx = dxr + k * 3;
+    const float* dv = dvr + k * 3;
+    const float zk = zr[k];
+    for (int i = 0; i < 3; ++i) {
+      go[i] += dx[i];
+      gd[i] += zk * dx[i] + dv[i];
+    }
+    if (is_depth[k >> 5] & (1u << (k & 31))) continue;
+    const float s = (zk - near) / span, g = dz_total(k);
+    g_near += g * (1.0f - s);
+    g_far += g * s;
+  }
+  float* o = d_rays + r * 8;
+  const float vals[8] = {go[0], go[1], go[2], gd[0], gd[1], gd[2], g_near, g_far};
+  for (int i = 0; i < 8; ++i) o[i] = accum ? o[i] + vals[i] : vals[i];
+}
+
+int launch_ray_grad(const float* rays, const float* z, const float* d_z, const float* d_xyz, const float* d_vd,
+                    const float* d_far_last, bool dz_has_pos, const float* depth, const float* nd, float depth_std,
+                    int Kfd, bool accum, float* d_rays, int64_t R, int K, cudaStream_t s) {
+  if (R == 0) return PNR_OK;
+  if (K > kMaxK) {
+    set_error("n_coarse + n_fine = %d exceeds %d", K, kMaxK);
+    return PNR_ERR_INVALID;
+  }
+  k_ray_grad<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(rays, z, d_z, d_xyz, d_vd, d_far_last, dz_has_pos ? 1 : 0,
+                                                         depth, nd, depth_std, Kfd, accum ? 1 : 0, d_rays, R, K);
+  PNR_LAUNCH_CHECK();
+  return PNR_OK;
+}
+
+// Backward of k_gen_rays (util.py:238-276): origin = P[:3, 3], dir = P[:3, :3] unproj (unit), so
+// d_P[:3, 3] += sum_pixels d_origin and d_P[:3, :3] += sum_pixels d_dir unproj^T.  One block per camera of the range
+// sums its pixels in a fixed order (thread-strided partial sums, then a shared-memory tree); one writer per pose.
+constexpr int kGenBwdThreads = 256;
+__global__ void __launch_bounds__(kGenBwdThreads) k_gen_rays_bwd(const float* __restrict__ d_rays, int W, int H,
+                                                                 float fx, float fy, float cx, float cy, int64_t first,
+                                                                 int64_t count, float* __restrict__ d_poses) {
+  __shared__ float red[12][kGenBwdThreads];
+  const int64_t hw = (int64_t)W * H;
+  const int64_t v = first / hw + blockIdx.x;
+  const int t = threadIdx.x;
+  int64_t a = v * hw, b = (v + 1) * hw;
+  if (a < first) a = first;
+  if (b > first + count) b = first + count;
+  float s[12];
+  for (int j = 0; j < 12; ++j) s[j] = 0.f;
+  for (int64_t i = a + t; i < b; i += kGenBwdThreads) {
+    const int rem = (int)(i - v * hw);
+    const int y = rem / W, x = rem - y * W;
+    const float X = ((float)x - cx) / fx;
+    const float Y = ((float)y - cy) / fy;
+    float dx = X, dy = -Y, dz = -1.0f;
+    const float n = sqrtf((dx * dx + dy * dy) + dz * dz);
+    const float u[3] = {dx / n, dy / n, dz / n};
+    const float* g = d_rays + (i - first) * 8;
+    for (int row = 0; row < 3; ++row) {
+      for (int col = 0; col < 3; ++col) s[row * 4 + col] += g[3 + row] * u[col];
+      s[row * 4 + 3] += g[row];
+    }
+  }
+  for (int j = 0; j < 12; ++j) red[j][t] = s[j];
+  __syncthreads();
+  for (int w = kGenBwdThreads / 2; w > 0; w >>= 1) {
+    if (t < w)
+      for (int j = 0; j < 12; ++j) red[j][t] += red[j][t + w];
+    __syncthreads();
+  }
+  if (t < 12) d_poses[v * 16 + t] += red[t][0];
+}
+
+int launch_gen_rays_bwd(const float* d_rays, int W, int H, float fx, float fy, float cx, float cy, int64_t first,
+                        int64_t count, float* d_poses, cudaStream_t s) {
+  if (count == 0) return PNR_OK;
+  const int64_t hw = (int64_t)W * H;
+  const int64_t nv = (first + count - 1) / hw - first / hw + 1;
+  k_gen_rays_bwd<<<(unsigned)nv, kGenBwdThreads, 0, s>>>(d_rays, W, H, fx, fy, cx, cy, first, count, d_poses);
+  PNR_LAUNCH_CHECK();
+  return PNR_OK;
 }
 
 int launch_depth_grad(const float* rays, const float* z_sorted, const float* depth, const float* nd,

@@ -4,9 +4,12 @@ Used whenever `net(xyz, ...)` itself is called with gradients required (a whole 
 `NeRFRenderer` uses the render-level node of render/fused_train.py instead; `PNR_FUSED_BACKWARD=1` forces this
 field-level node there too, `=0` the composed-torch path).  Validated on H100 (tests/test_gpu_backward.py).
 
-The autograd node takes the sample positions, the latent and the MLP parameters as inputs, so autograd carries
-`d_xyz` back into the renderer (sample depths), `d_latent` into the encoder trunk and the weight gradients into the
-optimiser, exactly where the reference's graph has them (train/train.py:199-215).
+The autograd node takes the sample positions, the view directions, the latent, the source cameras (`net.poses`,
+`net.focal`, `net.c`) and the MLP parameters as inputs, so autograd carries `d_xyz` / `d_viewdirs` back into the
+renderer (sample depths, rays), `d_latent` into the encoder trunk, the camera gradients to the poses / focal / c given
+to encode() and the weight gradients into the optimiser, exactly where the reference's graph has them
+(train/train.py:199-215, models.py:112-212).  Only the gradients autograd asks for are computed; without view-direction
+or camera gradients the backward is `pnr_field_backward`, otherwise `pnr_field_backward_cam`.
 """
 import torch
 
@@ -15,7 +18,7 @@ import pnr_native as pn
 
 class _FusedField(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, net, coarse, xyz, viewdirs, latent, *params):
+    def forward(ctx, net, coarse, xyz, viewdirs, latent, poses, focal, c, *params):
         ctx.net, ctx.coarse = net, coarse
         ctx.save_for_backward(xyz, viewdirs)
         with torch.no_grad():
@@ -43,15 +46,24 @@ class _FusedField(torch.autograd.Function):
         xyz_c = xyz.detach().contiguous().float()
         dirs_c = viewdirs.detach().reshape(SB, B, 3).contiguous().float()
         d_out_c = d_out.contiguous().float()
+        d_dirs = torch.empty(SB, B, 3, dtype=torch.float32, device=dev) if ctx.needs_input_grad[3] else None
+        cam, d_cam = pn.camera_grad(net, ctx.needs_input_grad[5:8], dev)
         L = pn.lib()
         nbytes = L.pnr_field_backward_workspace_bytes(scene, m, B)
         ws = pn.workspace(dev, nbytes)
         with torch.cuda.device(dev):
-            pn.check(L.pnr_field_backward(scene, m, pn.dptr(xyz_c, "xyz"), pn.dptr(dirs_c, "viewdirs"),
-                                          pn.dptr(d_out_c, "d_out"), gstruct, pn.dptr(d_latent), pn.dptr(d_xyz), B,
-                                          ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
+            if d_dirs is None and cam is None:
+                pn.check(L.pnr_field_backward(scene, m, pn.dptr(xyz_c, "xyz"), pn.dptr(dirs_c, "viewdirs"),
+                                              pn.dptr(d_out_c, "d_out"), gstruct, pn.dptr(d_latent), pn.dptr(d_xyz),
+                                              B, ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
+            else:
+                pn.check(L.pnr_field_backward_cam(scene, m, pn.dptr(xyz_c, "xyz"), pn.dptr(dirs_c, "viewdirs"),
+                                                  pn.dptr(d_out_c, "d_out"), gstruct, pn.dptr(d_latent),
+                                                  pn.dptr(d_xyz), pn.dptr(d_dirs), cam, B, ws.data_ptr(), ws.numel(),
+                                                  pn.stream_ptr(dev)))
         g_latent = d_latent.permute(0, 3, 1, 2) if want_latent else None
-        return (None, None, d_xyz, None, g_latent) + tuple(grads[k] for k in names)
+        g_dirs = d_dirs.reshape(viewdirs.shape) if d_dirs is not None else None
+        return (None, None, d_xyz, g_dirs, g_latent) + d_cam + tuple(grads[k] for k in names)
 
 
 def fused_field(net, xyz, coarse, viewdirs):
@@ -59,4 +71,4 @@ def fused_field(net, xyz, coarse, viewdirs):
     mlp = net.mlp_fine if use_fine else net.mlp_coarse
     latent = net.encoder.latent.detach() if net.stop_encoder_grad else net.encoder.latent
     params = [p for _, p in mlp.named_parameters()]
-    return _FusedField.apply(net, coarse, xyz, viewdirs, latent, *params)
+    return _FusedField.apply(net, coarse, xyz, viewdirs, latent, net.poses, net.focal, net.c, *params)

@@ -234,6 +234,8 @@ class PixelNeRFNet(torch.nn.Module):
             return True
         if self.encoder.latent.requires_grad:
             return True
+        if self.poses.requires_grad or self.focal.requires_grad or self.c.requires_grad:   # pose / intrinsics refinement
+            return True
         return any(p.requires_grad for p in self.mlp_coarse.parameters())
 
     # ------------------------------------------------------------------------------

@@ -59,6 +59,10 @@ class PnrRenderGrad(C.Structure):
                 ("d_rgb_fine", _fp), ("d_depth_fine", _fp), ("d_weights_fine", _fp)]
 
 
+class PnrCameraGrad(C.Structure):
+    _fields_ = [("d_poses", _fp), ("d_focal", _fp), ("d_c", _fp)]
+
+
 class PnrShard(C.Structure):
     _fields_ = [("scene", C.POINTER(PnrScene)), ("mlp_coarse", C.POINTER(PnrMlp)), ("mlp_fine", C.POINTER(PnrMlp)),
                 ("noise", C.POINTER(PnrNoise)), ("workspace", _fp), ("workspace_bytes", C.c_size_t),
@@ -70,6 +74,10 @@ class PnrShardGrad(C.Structure):
                 ("grad_coarse", C.POINTER(PnrMlp)), ("grad_fine", C.POINTER(PnrMlp)), ("d_latent_nhwc", _fp),
                 ("arena", _fp), ("arena_count", C.c_int64), ("arena_stage0", _fp),
                 ("workspace", _fp), ("workspace_bytes", C.c_size_t), ("stream", _fp)]
+
+
+class PnrShardCam(C.Structure):
+    _fields_ = [("cam", PnrCameraGrad), ("d_rays", _fp)]
 
 
 _lib = None
@@ -103,6 +111,15 @@ def declare(L):
     L.pnr_render_backward_ex.argtypes = [P(PnrScene), P(PnrMlp), P(PnrMlp), P(PnrRenderCfg), vp, P(PnrNoise),
                                          P(PnrRenderOut), P(PnrRenderGrad), P(PnrMlp), P(PnrMlp), vp, i64, vp, sz, vp]
     L.pnr_render_backward_ex.restype = C.c_int
+    L.pnr_field_backward_cam.argtypes = [P(PnrScene), P(PnrMlp), vp, vp, vp, P(PnrMlp), vp, vp, vp, P(PnrCameraGrad),
+                                         i64, vp, sz, vp]
+    L.pnr_field_backward_cam.restype = C.c_int
+    L.pnr_render_backward_cam.argtypes = [P(PnrScene), P(PnrMlp), P(PnrMlp), P(PnrRenderCfg), vp, P(PnrNoise),
+                                          P(PnrRenderOut), P(PnrRenderGrad), P(PnrMlp), P(PnrMlp), vp, vp,
+                                          P(PnrCameraGrad), i64, vp, sz, vp]
+    L.pnr_render_backward_cam.restype = C.c_int
+    L.pnr_gen_rays_backward.argtypes = [vp, vp, i64, i32, i32, f32, f32, f32, f32, i64, i64, vp, vp]
+    L.pnr_gen_rays_backward.restype = C.c_int
     L.pnr_composite_backward.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, i32, vp]
     L.pnr_composite_backward.restype = C.c_int
     L.pnr_render_workspace_bytes.argtypes = [P(PnrScene), P(PnrMlp), P(PnrMlp), P(PnrRenderCfg), i64]
@@ -128,9 +145,12 @@ def declare(L):
         L.pnr_mgpu_peer_load.restype = i32
         L.pnr_mgpu_render_backward.argtypes = [vp, P(PnrShard), P(PnrShardGrad), P(PnrRenderCfg), P(PnrRenderGrad),
                                                P(PnrMlp), P(PnrMlp), vp, i64, vp]
+        L.pnr_mgpu_render_backward_cam.argtypes = [vp, P(PnrShard), P(PnrShardGrad), P(PnrShardCam), P(PnrRenderCfg),
+                                                   P(PnrRenderGrad), P(PnrMlp), P(PnrMlp), vp, vp, P(PnrCameraGrad),
+                                                   i64, vp]
         L.pnr_sum_into.argtypes = [vp, P(vp), i32, i64, vp]
         for name in ("pnr_mgpu_create", "pnr_mgpu_destroy", "pnr_mgpu_broadcast", "pnr_mgpu_render",
-                     "pnr_mgpu_render_backward", "pnr_sum_into"):
+                     "pnr_mgpu_render_backward", "pnr_mgpu_render_backward_cam", "pnr_sum_into"):
             getattr(L, name).restype = C.c_int
     L.pnr_gemm_nt.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.pnr_gemm_nt.restype = C.c_int
@@ -198,6 +218,33 @@ def gen_rays(poses, width, height, fx, fy, cx, cy, z_near, z_far, first=0, count
                                  float(cy), float(z_near), float(z_far), int(first), int(count), dptr(out, "rays"),
                                  stream_ptr(poses.device)))
     return out
+
+
+class _GenRays(torch.autograd.Function):
+    """gen_rays with a gradient w.r.t. the camera-to-world poses: forward pnr_gen_rays, backward pnr_gen_rays_backward."""
+
+    @staticmethod
+    def forward(ctx, poses, width, height, fx, fy, cx, cy, z_near, z_far):
+        ctx.args = (poses.shape, poses.dtype, int(width), int(height), float(fx), float(fy), float(cx), float(cy))
+        p = poses.detach().to(torch.float32).contiguous()
+        ctx.save_for_backward(p)
+        return gen_rays(p, width, height, fx, fy, cx, cy, z_near, z_far)
+
+    @staticmethod
+    def backward(ctx, d_rays):
+        shape, dtype, W, H, fx, fy, cx, cy = ctx.args
+        (p,) = ctx.saved_tensors
+        d_rays = d_rays.to(torch.float32).contiguous()
+        d_poses = torch.zeros(p.shape, dtype=torch.float32, device=p.device)
+        with torch.cuda.device(p.device):
+            check(lib().pnr_gen_rays_backward(dptr(d_rays, "d_rays"), dptr(p, "poses"), p.shape[0], W, H, fx, fy, cx,
+                                              cy, 0, d_rays.shape[0], dptr(d_poses), stream_ptr(p.device)))
+        return (d_poses.to(dtype),) + (None,) * 8
+
+
+def gen_rays_autograd(poses, width, height, fx, fy, cx, cy, z_near, z_far):
+    """gen_rays of every pixel as an autograd node on `poses` (the same bits as gen_rays)."""
+    return _GenRays.apply(poses, width, height, fx, fy, cx, cy, z_near, z_far)
 
 
 def frames_u8(rgb, out=None):
@@ -297,6 +344,16 @@ def make_scene_struct(latent_nhwc, poses, focal, c, SB, NS, image_w, image_h, sc
     s.proj_coarse = dptr(proj_coarse)
     s.proj_fine = dptr(proj_fine)
     return s
+
+
+def camera_grad(net, needs, dev):
+    """PnrCameraGrad over zeroed buffers shaped as net.poses / net.focal / net.c, for those `needs` (three bools) asks
+    for -> (struct, or None when nothing is asked for; (d_poses, d_focal, d_c) with None for the rest)."""
+    ts = tuple(torch.zeros(t.shape, dtype=torch.float32, device=dev) if need else None
+               for t, need in zip((net.poses, net.focal, net.c), needs))
+    if all(t is None for t in ts):
+        return None, ts
+    return PnrCameraGrad(*(dptr(t) for t in ts)), ts
 
 
 def pack_latent(latent_nchw):

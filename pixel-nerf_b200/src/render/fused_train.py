@@ -12,9 +12,18 @@ rgb losses of train/train.py:199-212; the backward is `pnr_render_backward_ex` w
 output.  Outputs the loss does not use reach the backward as None and go to the library as NULL, so an rgb-only step
 runs the same arithmetic as the rgb-only entry point `pnr_render_backward`.
 
+The inputs are differentiable as in the reference's graph too: the rays (origin, direction, near, far) and the source
+cameras `net.poses` / `net.focal` / `net.c` that encode() derived with torch ops from the poses, focal and c it was
+given.  When any of them requires grad the backward is `pnr_render_backward_cam`, which also returns those gradients;
+autograd carries the pose gradient on to the camera-to-world poses given to encode() (and, through `util.gen_rays`, to
+the target poses of the rays).  So a frozen network can refine noisy poses.  Only the gradients autograd asks for are
+computed; with none of them asked for the call is `pnr_render_backward_ex`, unchanged.  `image_shape` and
+`latent_scaling` are buffers and get no gradient, as in the reference.
+
 `bind_parallel(net, gpus)` with several GPUs trains through `_ShardedFusedRender` below: the rays are sharded as by
 the reference's DataParallel(dim=1), every GPU renders and differentiates its shard, and the shards' gradients are
-summed onto gpus[0] (pnr_mgpu_render / pnr_mgpu_render_backward, csrc/pnr_mgpu.cu).
+summed onto gpus[0] (pnr_mgpu_render / pnr_mgpu_render_backward, csrc/pnr_mgpu.cu); with ray or camera gradients
+pnr_mgpu_render_backward_cam, whose camera gradients sit in the same per-shard arenas and are reduced with them.
 """
 import torch
 
@@ -25,7 +34,7 @@ from .dotmap_compat import DotMap
 
 class _FusedRender(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, renderer, model, want_weights, noise_in, rays, latent, *params):
+    def forward(ctx, renderer, model, want_weights, noise_in, rays, latent, poses, focal, c, *params):
         dev = rays.device
         SB, B, _ = rays.shape
         R = SB * B
@@ -106,17 +115,26 @@ class _FusedRender(torch.autograd.Function):
         ug = pn.PnrRenderGrad()
         for name, t in up.items():
             setattr(ug, name, pn.dptr(t, name))
+        d_rays = torch.empty(SB, B, 8, dtype=torch.float32, device=dev) if ctx.needs_input_grad[4] else None
+        cam, d_cam = pn.camera_grad(model, ctx.needs_input_grad[6:9], dev)
         nbytes = L.pnr_render_backward_workspace_bytes(scene, mc, mf, cfg, B)
         ws = pn.workspace(dev, nbytes)
+        gfine = gstructs[1] if len(gstructs) > 1 else None
         with torch.cuda.device(dev):
-            pn.check(L.pnr_render_backward_ex(scene, mc, mf, cfg, pn.dptr(rays, "rays"), noise, fwd, ug, gstructs[0],
-                                              gstructs[1] if len(gstructs) > 1 else None, pn.dptr(d_latent), B,
-                                              ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
+            if d_rays is None and cam is None:
+                pn.check(L.pnr_render_backward_ex(scene, mc, mf, cfg, pn.dptr(rays, "rays"), noise, fwd, ug,
+                                                  gstructs[0], gfine, pn.dptr(d_latent), B, ws.data_ptr(), ws.numel(),
+                                                  pn.stream_ptr(dev)))
+            else:
+                pn.check(L.pnr_render_backward_cam(scene, mc, mf, cfg, pn.dptr(rays, "rays"), noise, fwd, ug,
+                                                   gstructs[0], gfine, pn.dptr(d_latent), pn.dptr(d_rays), cam, B,
+                                                   ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
         g_latent = d_latent.permute(0, 3, 1, 2) if want_latent else None
         flat = []
         for mlp, g in zip(mlps, gdicts):
             flat += [g[k] for k, _ in mlp.named_parameters()]
-        return (None, None, None, None, None, g_latent) + tuple(flat)
+        return (None, None, None, None, d_rays, g_latent) + d_cam + tuple(flat)
+
 
 
 def fused_render_train(renderer, model, rays, want_weights, noise_in=None):
@@ -124,7 +142,8 @@ def fused_render_train(renderer, model, rays, want_weights, noise_in=None):
     mlps = [model.mlp_coarse] + ([model.mlp_fine] if (fine and model.mlp_fine is not None) else [])
     params = [p for mlp in mlps for _, p in mlp.named_parameters()]
     latent = model.encoder.latent.detach() if model.stop_encoder_grad else model.encoder.latent
-    outs = list(_FusedRender.apply(renderer, model, want_weights, noise_in, rays, latent, *params))
+    outs = list(_FusedRender.apply(renderer, model, want_weights, noise_in, rays, latent, model.poses, model.focal,
+                                   model.c, *params))
     res = DotMap()
     res.coarse = DotMap(rgb=outs.pop(0), depth=outs.pop(0))
     if want_weights:
@@ -142,13 +161,15 @@ def fused_render_train(renderer, model, rays, want_weights, noise_in=None):
 _WIDTHS = ("d_rgb_coarse", "d_depth_coarse", "d_weights_coarse", "d_rgb_fine", "d_depth_fine", "d_weights_fine")
 
 
-def _grad_arena(mlps, latent_shape, dev):
-    """One zeroed fp32 buffer on `dev` holding every parameter gradient of `mlps` and (latent_shape not None) the
-    channels-last latent gradient, so that one kernel reduces a shard's whole gradient -> (flat, [dict per mlp],
-    [PnrMlp per mlp], latent view or None).  Every device gets the same layout."""
+def _grad_arena(mlps, latent_shape, dev, cam_shapes=(None, None, None)):
+    """One zeroed fp32 buffer on `dev` holding every parameter gradient of `mlps`, (latent_shape not None) the
+    channels-last latent gradient and the camera gradients of `cam_shapes` (poses, focal, c; None = not wanted), so
+    that one kernel reduces a shard's whole gradient -> (flat, [dict per mlp], [PnrMlp per mlp], latent view or None,
+    (d_poses, d_focal, d_c) views or None).  Every device gets the same layout."""
     sizes = [p.numel() for mlp in mlps for _, p in mlp.named_parameters()]
     lat_n = 0 if latent_shape is None else torch.Size(latent_shape).numel()
-    flat = torch.zeros(sum(sizes) + lat_n, dtype=torch.float32, device=dev)
+    cam_n = [0 if sh is None else torch.Size(sh).numel() for sh in cam_shapes]
+    flat = torch.zeros(sum(sizes) + lat_n + sum(cam_n), dtype=torch.float32, device=dev)
     dicts, structs, off = [], [], 0
     for mlp in mlps:
         g = {}
@@ -158,8 +179,13 @@ def _grad_arena(mlps, latent_shape, dev):
         dicts.append(g)
         structs.append(pn.make_mlp_struct(g, mlp.d_in, mlp.d_latent, mlp.d_hidden, mlp.d_out, mlp.n_blocks,
                                           mlp.combine_layer))
-    lat = flat[off:].view(latent_shape) if latent_shape is not None else None
-    return flat, dicts, structs, lat
+    lat = flat[off:off + lat_n].view(latent_shape) if latent_shape is not None else None
+    off += lat_n
+    cams = []
+    for sh, k in zip(cam_shapes, cam_n):
+        cams.append(flat[off:off + k].view(sh) if sh is not None else None)
+        off += k
+    return flat, dicts, structs, lat, tuple(cams)
 
 
 class _ShardedFusedRender(torch.autograd.Function):
@@ -169,7 +195,7 @@ class _ShardedFusedRender(torch.autograd.Function):
     continues into the encoder there."""
 
     @staticmethod
-    def forward(ctx, sharded, want_weights, noise_in, rays, latent, *params):
+    def forward(ctx, sharded, want_weights, noise_in, rays, latent, poses, focal, c, *params):
         import ctypes as C
         net, renderer = sharded.module.net, sharded.module.renderer
         L = pn.lib()
@@ -260,7 +286,7 @@ class _ShardedFusedRender(torch.autograd.Function):
             pn.check(L.pnr_mgpu_render(sharded._mgpu(), shards, cfg, pn.dptr(rays0, "rays"), out0, B,
                                        pn.stream_ptr(dev0)))
         ctx.sharded, ctx.shards, ctx.keep, ctx.stages, ctx.bounds = sharded, shards, keep, stages, bounds
-        ctx.cfg, ctx.dims = cfg, (SB, B, Kc, Kf, fine)
+        ctx.cfg, ctx.dims, ctx.rays_device = cfg, (SB, B, Kc, Kf, fine), rays.device
         ctx.layout = [f"d_{q}_{p}" for p, q, _ in names]
         ctx.set_materialize_grads(False)     # unused outputs arrive as None -> NULL (zero) in PnrRenderGrad
         return tuple(outs)
@@ -282,7 +308,15 @@ class _ShardedFusedRender(torch.autograd.Function):
         mlps = [net.mlp_coarse] + ([net.mlp_fine] if (fine and net.mlp_fine is not None) else [])
         V, Cc, Hl, Wl = net.encoder.latent.shape
         lat_shape = (V, Hl, Wl, Cc) if ctx.needs_input_grad[4] else None
-        flat0, gdicts, gstructs, d_lat0 = _grad_arena(mlps, lat_shape, dev0)
+        cam_shapes = tuple(t.shape if need else None
+                           for t, need in zip((net.poses, net.focal, net.c), ctx.needs_input_grad[5:8]))
+        flat0, gdicts, gstructs, d_lat0, d_cam0 = _grad_arena(mlps, lat_shape, dev0, cam_shapes)
+        want_rays = ctx.needs_input_grad[3]
+        d_rays0 = torch.empty(SB, B, 8, dtype=torch.float32, device=dev0) if want_rays else None
+        cam0 = None
+        if any(t is not None for t in d_cam0):
+            cam0 = pn.PnrCameraGrad(*(pn.dptr(t) for t in d_cam0))
+        scs = (pn.PnrShardCam * n)()
         sgs = (pn.PnrShardGrad * n)()
         keep = [up, flat0]
         h = sharded._mgpu()
@@ -310,10 +344,15 @@ class _ShardedFusedRender(torch.autograd.Function):
                 ws = wss[gpus[i]]
                 sg.workspace, sg.workspace_bytes = ws.data_ptr(), ws.numel()
                 sg.stream = pn.stream_ptr(dev)
+                if want_rays and (i > 0 or SB > 1):      # the shard's ray gradients, un-staged onto gpus[0]
+                    dr = torch.empty(SB, Bi, 8, dtype=torch.float32, device=dev)
+                    scs[i].d_rays = pn.dptr(dr)
+                    keep.append(dr)
                 if i == 0:
                     sg.arena, sg.arena_count = pn.dptr(flat0), flat0.numel()
                     continue
-                flat, _, structs, d_lat = _grad_arena(mlps, lat_shape, dev)
+                flat, _, structs, d_lat, d_cam = _grad_arena(mlps, lat_shape, dev, cam_shapes)
+                scs[i].cam = pn.PnrCameraGrad(*(pn.dptr(t) for t in d_cam))
                 sg.grad_coarse = C.pointer(structs[0])
                 sg.grad_fine = C.pointer(structs[1]) if len(structs) > 1 else None
                 sg.d_latent_nhwc = pn.dptr(d_lat)
@@ -324,16 +363,22 @@ class _ShardedFusedRender(torch.autograd.Function):
                 sg.arena_stage0 = pn.dptr(stage0)
                 keep.append(stage0)
         keep.append(wss)
+        gfine = gstructs[1] if len(gstructs) > 1 else None
         with torch.cuda.device(dev0):
-            pn.check(L.pnr_mgpu_render_backward(h, ctx.shards, sgs, ctx.cfg, ug, gstructs[0],
-                                                gstructs[1] if len(gstructs) > 1 else None, pn.dptr(d_lat0), B,
-                                                pn.stream_ptr(dev0)))
+            if d_rays0 is None and cam0 is None:
+                pn.check(L.pnr_mgpu_render_backward(h, ctx.shards, sgs, ctx.cfg, ug, gstructs[0], gfine,
+                                                    pn.dptr(d_lat0), B, pn.stream_ptr(dev0)))
+            else:
+                pn.check(L.pnr_mgpu_render_backward_cam(h, ctx.shards, sgs, scs, ctx.cfg, ug, gstructs[0], gfine,
+                                                        pn.dptr(d_lat0), pn.dptr(d_rays0), cam0, B,
+                                                        pn.stream_ptr(dev0)))
         sharded._keep_bwd = keep     # (the driver also orders every shard stream after the reduction)
         g_latent = d_lat0.permute(0, 3, 1, 2) if d_lat0 is not None else None
         flat = []
         for mlp, g in zip(mlps, gdicts):
             flat += [g[k] for k, _ in mlp.named_parameters()]
-        return (None, None, None, None, g_latent) + tuple(flat)
+        g_rays = d_rays0.to(ctx.rays_device) if d_rays0 is not None else None
+        return (None, None, None, g_rays, g_latent) + d_cam0 + tuple(flat)
 
 
 def sharded_render_train(sharded, rays, want_weights, noise_in=None):
@@ -345,7 +390,8 @@ def sharded_render_train(sharded, rays, want_weights, noise_in=None):
     mlps = [net.mlp_coarse] + ([net.mlp_fine] if (fine and net.mlp_fine is not None) else [])
     params = [p for mlp in mlps for _, p in mlp.named_parameters()]
     latent = net.encoder.latent.detach() if net.stop_encoder_grad else net.encoder.latent
-    outs = list(_ShardedFusedRender.apply(sharded, want_weights, noise_in, rays, latent, *params))
+    outs = list(_ShardedFusedRender.apply(sharded, want_weights, noise_in, rays, latent, net.poses, net.focal, net.c,
+                                          *params))
     res = DotMap()
     res.coarse = DotMap(rgb=outs.pop(0), depth=outs.pop(0))
     if want_weights:

@@ -159,7 +159,8 @@ class _ShardedRender(torch.nn.Module):
     its own shard from the samples its forward left there, and one kernel on gpus[0] sums the shards' weight and latent
     gradients onto gpus[0]'s, so autograd continues into the encoder there as under DataParallel.  The optimizer step
     and encode() change the weights and the scene on every step, so every step refreshes the replicas.  Other models,
-    CPU rays or PNR_FUSED_BACKWARD=0/1 run the step on gpus[0] alone, with a one-time warning."""
+    CPU rays or PNR_FUSED_BACKWARD=0/1 run the step on gpus[0] alone, with a one-time warning.  Gradients of the rays
+    and the cameras (poses, focal, c) are sharded too (pnr_mgpu_render_backward_cam)."""
 
     def __init__(self, wrapped, gpus):
         super().__init__()

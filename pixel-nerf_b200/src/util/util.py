@@ -60,13 +60,21 @@ def unproj_map(width, height, f, c=None, device="cpu"):
 
 
 def gen_rays(poses, width, height, focal, z_near, z_far, c=None, ndc=False):
-    """(NV,4,4) camera-to-world -> (NV,H,W,8) [origin, unit dir, near, far] (util.py:238-276)."""
+    """(NV,4,4) camera-to-world -> (NV,H,W,8) [origin, unit dir, near, far] (util.py:238-276).
+
+    Differentiable w.r.t. `poses` as in the reference: on CUDA, with grad mode on and `poses.requires_grad`, the kernel
+    runs inside an autograd node whose backward is `pnr_gen_rays_backward`.  The reference reads focal and c as Python
+    floats (util.py:134-139), so neither gets a gradient through the rays, here as there."""
     if ndc:
         raise NotImplementedError("NDC rays are not used by any shipped config")
     nv, dev = poses.shape[0], poses.device
     if dev.type == "cuda":     # poses already on the GPU: the pnr_gen_rays kernel (no CPU detour)
         import pnr_native
-        fx, fy, cx, cy = _intrinsics(width, height, torch.as_tensor(focal).squeeze(), c)
+        fx, fy, cx, cy = _intrinsics(width, height, torch.as_tensor(focal).detach().squeeze(),
+                                     c.detach() if torch.is_tensor(c) else c)
+        if torch.is_grad_enabled() and poses.requires_grad:
+            rays = pnr_native.gen_rays_autograd(poses, width, height, fx, fy, cx, cy, z_near, z_far)
+            return rays.view(nv, height, width, 8)
         return pnr_native.gen_rays(poses, width, height, fx, fy, cx, cy, z_near, z_far).view(nv, height, width, 8)
     cam = unproj_map(width, height, torch.as_tensor(focal).squeeze(), c=c, device=dev)
     dirs = torch.matmul(poses[:, None, None, :3, :3], cam[None].expand(nv, -1, -1, -1).unsqueeze(-1))[..., 0]

@@ -5,6 +5,7 @@ with want_weights=True, MSE coarse + MSE fine, backward through MLPs and the enc
 
     python scripts/bench_train.py --mode render     # the package default: pnr_render + pnr_render_backward in one node
     python scripts/bench_train.py --mode field      # PNR_FUSED_BACKWARD=1: torch renderer, fused field fwd + pnr_field_backward
+    python scripts/bench_train.py --cam-grad        # + backward device ms with ray / camera gradients (frozen net too)
     python scripts/bench_train.py --mode torch      # PNR_FUSED_BACKWARD=0: composed-torch grad path of this package
     python scripts/bench_train.py --mode reference  # the UNMODIFIED reference (oracle/_ref), same step, same GPU
     python scripts/bench_train.py --gpus "0 1"      # render mode through bind_parallel(net, [0, 1]): rays sharded over
@@ -37,6 +38,8 @@ def main():
     ap.add_argument("--B", type=int, default=128)
     ap.add_argument("--tiny", action="store_true", help="d_hidden 32, 8+4 samples, 32x32 images: a script self-check")
     ap.add_argument("--gpus", default=None, help='device ids as train.py\'s --gpu_id, e.g. "0 1" (render mode)')
+    ap.add_argument("--cam-grad", action="store_true",
+                    help="render mode, one GPU: device ms of the backward with and without ray / camera gradients")
     a = ap.parse_args()
     gpus = [int(x) for x in a.gpus.split()] if a.gpus else None
     if gpus:
@@ -134,6 +137,8 @@ def main():
     res = {"metric": "training rays/s (encode + render fwd/bwd + Adam)", "mode": a.mode,
            "value": SB * B * a.steps / dt, "ms_per_step": dt / a.steps * 1e3, "SB": SB, "B": B,
            "loss_first": losses[0], "loss_last": losses[-1], "finite": bool(np.isfinite(losses).all())}
+    if a.cam_grad:
+        res.update(gpu=torch.cuda.get_device_name(dev), **cam_grad_ms(net, render_par, batch, focal, dev, a))
     if gpus:
         # device ms per step on the first GPU's stream (forward includes the replica refresh, backward the reduction)
         per_step = lambda evs: sum(e[0].elapsed_time(e[1]) for e in evs) / a.steps
@@ -141,6 +146,36 @@ def main():
                    forward_ms=per_step(timing["forward"]), backward_ms=per_step(timing["backward"]),
                    refresh_ms=per_step(timing.get("refresh", [])), reduction_ms=reduction_ms(net, gpus, dev, a.steps))
     print(json.dumps(res))
+
+
+def cam_grad_ms(net, render_par, batch, focal, dev, a):
+    """Device ms of loss.backward() per step (CUDA events on the current stream) for the same step three ways: the
+    training step above ("train"), the same with the rays and the source poses requiring grad ("train_cam"), and a
+    frozen network (encoder and MLPs) with only the rays and the source poses requiring grad ("frozen_cam")."""
+    out = {}
+    for name in ("train", "train_cam", "frozen_cam"):
+        net.requires_grad_(name != "frozen_cam")
+        evs = []
+        for i in range(a.warmup + a.steps):
+            images, src, rays, gt = batch()
+            if name != "train":
+                src.requires_grad_(True)
+                rays.requires_grad_(True)
+            net.encode(images, src, focal.to(dev))
+            res = render_par(rays, want_weights=True)
+            loss = torch.nn.functional.mse_loss(res["coarse"]["rgb"], gt) + torch.nn.functional.mse_loss(
+                res["fine"]["rgb"], gt)
+            net.zero_grad(set_to_none=True)
+            ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            ev[0].record()
+            loss.backward()
+            ev[1].record()
+            if i >= a.warmup:
+                evs.append(ev)
+        torch.cuda.synchronize(dev)
+        out[f"backward_ms_{name}"] = sum(e[0].elapsed_time(e[1]) for e in evs) / len(evs)
+    net.requires_grad_(True)
+    return out
 
 
 def reduction_ms(net, gpus, dev, reps):

@@ -379,6 +379,38 @@ int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrSh
  * j < count.  src: host array of n <= 63 device pointers readable from the current device. */
 int pnr_sum_into(float* dst, const float* const* src, int32_t n, int64_t count, void* stream);
 
+/* ---- mesh extraction: util/recon.py marching_cubes (src/util/recon.py:12-78) ------------------------------------ */
+
+/* The evaluation grid of recon.py:43, util.gen_grid(*zip(lo, hi, reso), ij_indexing=True) (src/util/util.py:93-110):
+ * points [first, first+count) of the nx*ny*nz grid in ij order (x slowest) -> xyz [count][3].  Each axis is
+ * np.linspace(lo, hi, n, dtype=float32): computed in float64 with the last point set to hi, then rounded, so the
+ * points are bit-equal to the reference's.  viewdirs (may be NULL) [count][3] = -p / |p| in fp32 (recon.py:54, with
+ * |p| = sqrt((x*x + y*y) + z*z) as torch's CPU norm sums it there, so the bits agree too); a grid point at the origin
+ * gets NaN there, as in the reference.
+ * lo, hi (double[3]) and reso (int32[3], each >= 1) are HOST arrays. */
+int pnr_grid_points(const double* lo, const double* hi, const int32_t* reso, int64_t first, int64_t count, float* xyz,
+                    float* viewdirs, void* stream);
+
+/* Marching cubes over a dense fp32 volume vol [nx][ny][nz] (what recon.py:68 `sigmas.view(*reso)` is), in two phases
+ * so that the caller can size the outputs exactly:
+ *   pnr_mc_count: counts_out[0] = vertices, counts_out[1] = triangles (int64, DEVICE memory); leaves in the workspace
+ *                 the edge flags, vertex ids, cell configurations and triangle offsets that pnr_mc_emit reads.
+ *   pnr_mc_emit : same vol / dims / iso / workspace, after pnr_mc_count on the same stream ->
+ *                 verts [n_verts][3] float64, tris [n_tris][3] int64 vertex ids (n_* = the counted values).
+ * A corner is inside when it is finite and sigma > iso.  One vertex per grid edge whose corners differ, numbered in
+ * (grid point, axis) order and shared by every cell touching the edge (the mesh is welded), at the lower corner's grid
+ * index plus t = (iso - s_a) / (s_b - s_a) along the edge in float64 (0.5 when the outside corner is NaN or infinite).  Triangles
+ * come from generated tables (oracle/make_mc_tables.py), cells in linear order, counter-clockwise seen from outside
+ * the inside region (normals toward decreasing sigma); every face is resolved from its own four corners, so the
+ * surface is watertight.  Offsets are exclusive scans (no atomics): repeated calls give the same bits.
+ * A dimension below 2 gives no cells, vertices or triangles.  Errors: dimensions < 1 or above 2^36 points, negative
+ * sizes, NULL pointers -> PNR_ERR_INVALID; workspace < pnr_mc_workspace_bytes -> PNR_ERR_WORKSPACE. */
+size_t pnr_mc_workspace_bytes(int32_t nx, int32_t ny, int32_t nz);
+int pnr_mc_count(const float* vol, int32_t nx, int32_t ny, int32_t nz, double iso, int64_t* counts_out,
+                 void* workspace, size_t workspace_bytes, void* stream);
+int pnr_mc_emit(const float* vol, int32_t nx, int32_t ny, int32_t nz, double iso, double* verts, int64_t* tris,
+                int64_t n_verts, int64_t n_tris, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.
  * engine = PNR_ENGINE_SIMT: fp32 FFMA SGEMM; PNR_ENGINE_TC (or AUTO): split-bf16 wgmma GEMM (3 products, fp32

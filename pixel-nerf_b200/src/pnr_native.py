@@ -152,6 +152,15 @@ def declare(L):
         for name in ("pnr_mgpu_create", "pnr_mgpu_destroy", "pnr_mgpu_broadcast", "pnr_mgpu_render",
                      "pnr_mgpu_render_backward", "pnr_mgpu_render_backward_cam", "pnr_sum_into"):
             getattr(L, name).restype = C.c_int
+    if hasattr(L, "pnr_grid_points"):     # (the host-emulator build of tests/cuda_emu has no mesh extraction)
+        f64 = C.c_double
+        L.pnr_grid_points.argtypes = [P(f64), P(f64), P(i32), i64, i64, vp, vp, vp]
+        L.pnr_mc_workspace_bytes.argtypes = [i32, i32, i32]
+        L.pnr_mc_workspace_bytes.restype = sz
+        L.pnr_mc_count.argtypes = [vp, i32, i32, i32, f64, vp, vp, sz, vp]
+        L.pnr_mc_emit.argtypes = [vp, i32, i32, i32, f64, vp, vp, i64, i64, vp, sz, vp]
+        for name in ("pnr_grid_points", "pnr_mc_count", "pnr_mc_emit"):
+            getattr(L, name).restype = C.c_int
     L.pnr_gemm_nt.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.pnr_gemm_nt.restype = C.c_int
     L.pnr_profile_begin.restype = C.c_int
@@ -257,6 +266,41 @@ def frames_u8(rgb, out=None):
     with torch.cuda.device(rgb.device):
         check(lib().pnr_frames_u8(dptr(rgb, "rgb"), rgb.numel(), C.c_void_p(out.data_ptr()), stream_ptr(rgb.device)))
     return out
+
+
+def grid_points(lo, hi, reso, first, count, xyz, viewdirs=None):
+    """pnr_grid_points: points [first, first+count) of util.gen_grid(*zip(lo, hi, reso), ij_indexing=True) into
+    xyz [>= count, 3] (and -p/|p| into viewdirs), both contiguous fp32 CUDA tensors."""
+    for t, name in ((xyz, "xyz"), (viewdirs, "viewdirs")):
+        if t is not None and (t.dim() != 2 or t.shape[0] < count or t.shape[1] != 3):
+            raise RuntimeError(f"grid_points: {name} must be [>= {count}, 3], got {tuple(t.shape)}")
+    dev = xyz.device
+    with torch.cuda.device(dev):
+        check(lib().pnr_grid_points((C.c_double * 3)(*map(float, lo)), (C.c_double * 3)(*map(float, hi)),
+                                    (C.c_int32 * 3)(*map(int, reso)), int(first), int(count), dptr(xyz, "xyz"),
+                                    dptr(viewdirs, "viewdirs"), stream_ptr(dev)))
+
+
+def marching_cubes(vol, iso):
+    """pnr_mc_count + pnr_mc_emit on a contiguous fp32 CUDA volume (nx, ny, nz) -> (vertices float64 [N, 3] in grid
+    index space, triangles int64 [M, 3]), CUDA tensors on vol's device.  Synchronises once, to size the outputs."""
+    if vol.dim() != 3:
+        raise RuntimeError(f"marching_cubes: expected a 3-D volume, got shape {tuple(vol.shape)}")
+    nx, ny, nz = vol.shape
+    dev = vol.device
+    L = lib()
+    ws = torch.empty(max(int(L.pnr_mc_workspace_bytes(nx, ny, nz)), 1), dtype=torch.uint8, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        s = stream_ptr(dev)
+        check(L.pnr_mc_count(dptr(vol, "vol"), nx, ny, nz, float(iso), C.c_void_p(counts.data_ptr()),
+                             C.c_void_p(ws.data_ptr()), ws.numel(), s))
+        nv, nt = counts.tolist()
+        verts = torch.empty(nv, 3, dtype=torch.float64, device=dev)
+        tris = torch.empty(nt, 3, dtype=torch.int64, device=dev)
+        check(L.pnr_mc_emit(dptr(vol, "vol"), nx, ny, nz, float(iso), C.c_void_p(verts.data_ptr()),
+                            C.c_void_p(tris.data_ptr()), nv, nt, C.c_void_p(ws.data_ptr()), ws.numel(), s))
+    return verts, tris
 
 
 def profile_begin():

@@ -1,0 +1,97 @@
+"""
+Mesh reconstruction tools (the reference's src/util/recon.py), on the GPU.
+
+`marching_cubes` evaluates sigma on a grid with the fused field kernels and extracts the isosurface with the
+library's own marching cubes (`pnr_grid_points`, `pnr_field_eval`, `pnr_mc_count` / `pnr_mc_emit`, include/pnr.h):
+the grid, the sigma volume and the mesh stay on the device, and only the mesh comes back.  There is no CPU path.
+"""
+import warnings
+
+import numpy as np
+import torch
+
+import pnr_native as pn
+
+
+def marching_cubes(
+    occu_net,
+    c1=[-1, -1, -1],
+    c2=[1, 1, 1],
+    reso=[128, 128, 128],
+    isosurface=50.0,
+    sigma_idx=3,
+    eval_batch_size=100000,
+    coarse=True,
+    device=None,
+):
+    """
+    Run marching cubes on network.
+    WARNING: does not make much sense with viewdirs in current form, since
+    sigma depends on viewdirs.
+    :param occu_net main NeRF type network, encoded with one object (num_objs == 1), on a CUDA device
+    :param c1 corner 1 of marching cube bounds x,y,z
+    :param c2 corner 2 of marching cube bounds x,y,z (all > c1)
+    :param reso resolutions of marching cubes x,y,z
+    :param isosurface sigma-isosurface of marching cubes
+    :param sigma_idx index of 'sigma' value in last dimension of occu_net's output
+    :param eval_batch_size batch size for evaluation
+    :param coarse whether to use coarse NeRF for evaluation
+    :param device optionally, device to put points for evaluation.
+    By default uses device of occu_net's first parameter.
+    :return vertices (N, 3) float64 numpy, scaled as vertex index * (c2 - c1) / reso + c1; triangles (M, 3) int64
+    numpy of vertex ids, counter-clockwise seen from outside (normals toward decreasing sigma)
+    """
+    if occu_net.use_viewdirs:
+        warnings.warn(
+            "Running marching cubes with fake view dirs (pointing to origin), output may be invalid"
+        )
+    if occu_net.num_objs != 1:
+        raise RuntimeError(f"marching_cubes needs a network encoded with one object, got num_objs = {occu_net.num_objs}")
+    if device is None:
+        device = next(occu_net.parameters()).device
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise RuntimeError(f"marching_cubes runs on CUDA only (no CPU fallback); got device {device}")
+    reso = [int(r) for r in reso]
+    N = reso[0] * reso[1] * reso[2]
+    is_train = occu_net.training
+    occu_net.eval()
+    try:
+        with torch.no_grad():
+            print("Evaluating sigma @", N, "points")
+            bs = max(1, min(int(eval_batch_size), N))
+            pts = torch.empty(bs, 3, dtype=torch.float32, device=device)
+            vd = torch.empty(bs, 3, dtype=torch.float32, device=device)
+            sigmas = torch.empty(N, dtype=torch.float32, device=device)
+            for first in range(0, N, bs):
+                n = min(bs, N - first)
+                pn.grid_points(c1, c2, reso, first, n, pts, vd)
+                out = occu_net(pts[None, :n], coarse=coarse, viewdirs=vd[None, :n])
+                sigmas[first:first + n] = out[0, :, sigma_idx]
+
+            print("Running marching cubes")
+            vertices, triangles = pn.marching_cubes(sigmas.view(*reso), isosurface)
+            vertices, triangles = vertices.cpu().numpy(), triangles.cpu().numpy()
+    finally:
+        if is_train:
+            occu_net.train()
+    # Scale (by reso, not reso - 1, as the reference does)
+    c1, c2 = np.array(c1), np.array(c2)
+    vertices *= (c2 - c1) / np.array(reso)
+    return vertices + c1, triangles
+
+
+def save_obj(vertices, triangles, path, vert_rgb=None):
+    """
+    Save an OBJ file: one `v x y z` line per vertex (`v x y z r g b` with per-vertex colours), then one 1-based
+    `f a b c` line per triangle; every coordinate and colour with %.4f.
+    :param vertices (N, 3)
+    :param triangles (M, 3) 0-based vertex ids
+    :param vert_rgb (N, 3) rgb, optional
+    """
+    vertices = np.asarray(vertices)
+    rows = vertices if vert_rgb is None else np.concatenate([vertices, np.asarray(vert_rgb)], axis=1)
+    vfmt = "v" + " %.4f" * rows.shape[1] + "\n"
+    with open(path, "w") as f:
+        f.writelines(vfmt % tuple(r) for r in rows)
+        f.writelines("f %d %d %d\n" % (a + 1, b + 1, c + 1) for a, b, c in np.asarray(triangles))

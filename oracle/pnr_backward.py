@@ -34,6 +34,12 @@ def _mm(a, b):
     return a @ b
 
 
+def _linear(x, w, b):
+    """Every layer of field_forward_saved goes through here (tests/test_gpu_backward_wide.py swaps in the split-bf16
+    operands of the CUDA backward's recomputed forward)."""
+    return F.linear(x, w, b)
+
+
 # ----------------------------------------------------------------------------------------
 # compositing (nerf.py:178-182, 222-249)
 # ----------------------------------------------------------------------------------------
@@ -92,19 +98,19 @@ def field_forward_saved(xyz, viewdirs, state, latent, w, NS, n_blocks=5, combine
     sv = dict(SB=SB, P=P, NS=NS, R=R, x_rot=x_rot.reshape(-1, 3), x_cam=x_cam, uv=uv, feat=zf, lat=lat,
               latent_shape=latent.shape, n_blocks=n_blocks, combine_layer=combine_layer, w=w, state=state,
               latent=latent, blocks=[])
-    h = F.linear(zf, w["lin_in.weight"], w["lin_in.bias"])
+    h = _linear(zf, w["lin_in.weight"], w["lin_in.bias"])
     for b in range(n_blocks):
         if b == combine_layer and NS > 1:
             h = h.reshape(-1, NS, P, h.shape[-1]).mean(dim=1).reshape(-1, h.shape[-1])
         if b < combine_layer:
-            h = h + F.linear(lat, w[f"lin_z.{b}.weight"], w[f"lin_z.{b}.bias"])
+            h = h + _linear(lat, w[f"lin_z.{b}.weight"], w[f"lin_z.{b}.bias"])
         a = torch.relu(h)
-        n = F.linear(a, w[f"blocks.{b}.fc_0.weight"], w[f"blocks.{b}.fc_0.bias"])
+        n = _linear(a, w[f"blocks.{b}.fc_0.weight"], w[f"blocks.{b}.fc_0.bias"])
         r = torch.relu(n)
         sv["blocks"].append(dict(h_pre=h, a=a, n=n, r=r))
-        h = h + F.linear(r, w[f"blocks.{b}.fc_1.weight"], w[f"blocks.{b}.fc_1.bias"])
+        h = h + _linear(r, w[f"blocks.{b}.fc_1.weight"], w[f"blocks.{b}.fc_1.bias"])
     sv["h_last"] = h
-    o4 = F.linear(torch.relu(h), w["lin_out.weight"], w["lin_out.bias"]).reshape(SB, P, 4)
+    o4 = _linear(torch.relu(h), w["lin_out.weight"], w["lin_out.bias"]).reshape(SB, P, 4)
     sv["o4"] = o4
     out = torch.cat((torch.sigmoid(o4[..., :3]), torch.relu(o4[..., 3:4])), dim=-1)
     return out, sv

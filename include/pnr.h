@@ -144,6 +144,26 @@ typedef struct PnrCameraGrad {
 int pnr_abi_version(void);
 const char* pnr_last_error(void);
 
+/* Deterministic mode, a flag of the calling thread (like pnr_last_error), 0 by default.  pnr_set_deterministic sets
+ * it (nonzero = on) and returns the previous value.  With it on, the calls of this thread give the same bits run to
+ * run on the same device and inputs:
+ *   - the tensor-core GEMMs (field backward, pnr_project_latent) sum split-K partial tiles in split order from a
+ *     partial buffer in the caller's workspace, instead of adding them with float atomics;
+ *   - the field backward adds the latent gradient per chunk in 64-bit fixed point (integer atomics, exact and
+ *     order-free) and converts it into d_latent_nhwc once per chunk.  A non-finite term makes every d_latent element
+ *     it reaches NaN.
+ * pnr_field_backward_workspace_bytes and pnr_render_backward_workspace_bytes report the extra space when the calling
+ * thread's flag is set, so set it before the size query.  With the flag off every call is unchanged. */
+int pnr_set_deterministic(int on);
+int pnr_get_deterministic(void);
+
+/* Backward of bilinear upsampling with align_corners=True (torch.nn.functional.interpolate):
+ * d_out [N][C][h_out][w_out] -> d_in [N][C][h_in][w_in] (overwritten), contiguous fp32.  A gather: each input pixel
+ * sums, in output order, the terms (tap weight products as torch computes them) of the output pixels that read it,
+ * so the result does not depend on scheduling.  Same-size maps copy. */
+int pnr_upsample_bilinear_ac_backward(const float* d_out, int64_t N, int32_t C, int32_t h_in, int32_t w_in,
+                                      int32_t h_out, int32_t w_out, float* d_in, void* stream);
+
 /* NCHW -> channels-last copy of the encoder latent (replaces the strided gather +
  * transpose of encoder.py:102-108 / models.py:219).  src [V][C][Hl][Wl] -> dst [V][Hl][Wl][C]. */
 int pnr_pack_latent(const float* latent_nchw, float* latent_nhwc, int32_t V, int32_t C, int32_t Hl,
@@ -286,7 +306,8 @@ int pnr_render(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* ml
  *    (128 output rows x 64 k, in the order the fused kernel consumes them).
  *  - pnr_project_latent: proj[i][v][y][x][:] = lin_z[i](latent[v,:,y,x]) (+ bias), so that the
  *    per-sample lin_z GEMMs (resnetfc.py:175) become a bilinear gather of the projected map
- *    (bilinear interpolation commutes with a linear layer). */
+ *    (bilinear interpolation commutes with a linear layer).  In deterministic mode the workspace beyond its first
+ *    3 * d_hidden floats (+ 256 B) holds the GEMM's split-K partials; 64 MiB more covers every shipped shape. */
 size_t pnr_pack_mlp_bytes(const PnrMlp* mlp);
 int pnr_pack_mlp(const PnrMlp* mlp, void* packed, size_t packed_bytes, void* stream);
 size_t pnr_project_latent_bytes(const PnrScene* scene, const PnrMlp* mlp);

@@ -23,6 +23,11 @@ void set_error(const char* fmt, ...) {
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
+static thread_local int g_deterministic = 0;
+static thread_local SplitKScratch g_splitk{nullptr, 0};
+bool deterministic() { return g_deterministic != 0; }
+SplitKScratch& splitk_scratch() { return g_splitk; }
+
 int sgemm(const float* A, int lda, const float* W, const float* bias, float* C, int ldc, int M, int N, int K,
           bool relu_a, bool accum, cudaStream_t s);                 // pnr_field_simt.cu
 int gemm_bf16x3(const float* A, int lda, const float* W, int ldw, const float* bias, float* C, int ldc, int M, int N,
@@ -118,6 +123,13 @@ extern "C" {
 int pnr_abi_version(void) { return PNR_ABI_VERSION; }
 const char* pnr_last_error(void) { return g_err; }
 int64_t pnr_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
+
+int pnr_set_deterministic(int on) {
+  const int prev = g_deterministic;
+  g_deterministic = on ? 1 : 0;
+  return prev;
+}
+int pnr_get_deterministic(void) { return g_deterministic; }
 
 int pnr_profile_begin(void) {
   for (cudaEvent_t e : g_prof_ev) g_prof_pool.push_back(e);

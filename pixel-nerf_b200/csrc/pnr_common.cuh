@@ -44,6 +44,24 @@ void prof_after(cudaStream_t s);
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// ---- deterministic mode (pnr_set_deterministic; pnr_api.cu) -----------------------------
+// The calling thread's flag.  When set, the training path uses its fixed-order variants: ordered split-K in the
+// tensor-core GEMM and the fixed-point latent scatter of the field backward.
+bool deterministic();
+// Partial tiles of the ordered split-K, carved from the caller's workspace by the entry point that runs the GEMMs and
+// installed for the duration of its call (SplitKScope).  A GEMM in deterministic mode splits K no further than this
+// buffer holds; with none installed it does not split.
+struct SplitKScratch {
+  float* p;
+  size_t bytes;
+};
+SplitKScratch& splitk_scratch();
+struct SplitKScope {
+  SplitKScratch saved;
+  SplitKScope(float* p, size_t bytes) : saved(splitk_scratch()) { splitk_scratch() = SplitKScratch{p, bytes}; }
+  ~SplitKScope() { splitk_scratch() = saved; }
+};
+
 // Bump allocator over the caller's workspace.
 struct Arena {
   char* base;

@@ -27,6 +27,10 @@ int gemm_bf16x3_masked(const float* A, int lda, const float* W, int ldw, float* 
                        const float* mask, cudaStream_t s);
 __global__ void k_pad_rows(const float* __restrict__ src, float* __restrict__ dst, int rows, int k_src, int k_dst);
 __global__ void k_view_mean(const float* __restrict__ X, float* __restrict__ Y, int64_t n_pts, int NS, int d);
+// pnr_determ.cu (deterministic mode).  Weak, so that a build without that unit (the host emulator of the SIMT units)
+// still links; there deterministic mode reports itself unavailable.
+int latent_scatter_fixed(const PnrScene& sc, const PointSource& src, int64_t g0, int64_t n, const float* d_lat,
+                         float* d_latent, long long* acc, unsigned* m_bits, cudaStream_t s) __attribute__((weak));
 
 namespace bwd {
 
@@ -200,6 +204,8 @@ __global__ void k_geom_bwd(PnrScene sc, PointSource src, int64_t g0, int64_t n_p
   const int C = sc.C, Wl = sc.Wl, Hl = sc.Hl;
   for (int v = 0; v < sc.NS; ++v) {
     const int64_t row = lp * sc.NS + v;
+    // the tap arithmetic below (to w_se) is restated by bwd_taps (pnr_geom.cuh) for deterministic mode's scatter:
+    // change both together
     const float* M = sc.poses + (size_t)(sb * sc.NS + v) * 12;
     float q[3], p[3];
     for (int i = 0; i < 3; ++i) {
@@ -365,10 +371,24 @@ static int64_t chunk_points(const PnrScene& sc, int64_t total_points) {
 struct Bufs {
   float *feat, *lat, *latT, *featT, *hpre[PNR_MAX_BLOCKS], *nbuf[PNR_MAX_BLOCKS], *xv, *hlast, *dh, *dhv, *T, *T2, *tA, *tB,
       *dlat, *dfeat, *do4, *w_in, *w_inT, *tmp_win, *w0T[PNR_MAX_BLOCKS], *w1T[PNR_MAX_BLOCKS], *wzT[PNR_MAX_BLOCKS],
-      *cam_acc;
+      *cam_acc, *splitk;
+  long long* lat_fixed;
+  unsigned* m_bits;
+  size_t splitk_bytes;
 };
 
-static size_t carve(Arena& ar, Bufs& b, const PnrScene& sc, const PnrMlp& mlp, int64_t cp) {
+// Deterministic mode's split-K partials: a split GEMM covers splits * tiles <= 2 * SMs + tiles - 1 < 3 * SMs output
+// tiles of 128 x 128, and never has more splits than K / 256.  Sized for the 132 SMs of an H100 SXM (a GPU with more
+// splits less) and for this call's shapes.
+static size_t splitk_budget(int64_t R, int d, int L) {
+  const int64_t w = d > L ? (d > 48 ? d : 48) : (L > 48 ? L : 48);
+  const int64_t dw = (pad16((int)R) / 256) * w * w, dx = (w / 256) * R * w, cap = (int64_t)3 * 132 * 128 * 128;
+  int64_t e = dw > dx ? dw : dx;
+  if (e > cap) e = cap;
+  return (size_t)e * sizeof(float);
+}
+
+static size_t carve(Arena& ar, Bufs& b, const PnrScene& sc, const PnrMlp& mlp, int64_t cp, bool det) {
   const size_t R = (size_t)cp * sc.NS, d = mlp.d_hidden, L = mlp.d_latent, Rp = pad16((int)R);
   b.feat = ar.take<float>(R * 48);
   b.lat = ar.take<float>(R * L);
@@ -396,6 +416,10 @@ static size_t carve(Arena& ar, Bufs& b, const PnrScene& sc, const PnrMlp& mlp, i
   b.w_inT = ar.take<float>(48 * d);
   b.tmp_win = ar.take<float>(d * 48);
   b.cam_acc = ar.take<float>((size_t)sc.SB * sc.NS * 16);
+  b.splitk_bytes = det ? splitk_budget((int64_t)R, (int)d, (int)L) : 0;
+  b.splitk = det ? ar.take<float>(b.splitk_bytes / sizeof(float)) : nullptr;
+  b.lat_fixed = det ? ar.take<long long>((size_t)sc.SB * sc.NS * sc.Hl * sc.Wl * sc.C) : nullptr;
+  b.m_bits = det ? ar.take<unsigned>(1) : nullptr;
   return ar.off;
 }
 
@@ -404,7 +428,7 @@ static size_t carve(Arena& ar, Bufs& b, const PnrScene& sc, const PnrMlp& mlp, i
 size_t field_backward_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int64_t total_points) {
   Arena ar(nullptr, (size_t)-1);
   bwd::Bufs b;
-  return bwd::carve(ar, b, sc, mlp, bwd::chunk_points(sc, total_points)) + 4096;
+  return bwd::carve(ar, b, sc, mlp, bwd::chunk_points(sc, total_points), deterministic()) + 4096;
 }
 
 #define BW(expr)                \
@@ -431,10 +455,16 @@ int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src
     set_error("workspace too small: %zu < %zu", ws_bytes, field_backward_workspace_bytes(sc, mlp, total_points));
     return PNR_ERR_WORKSPACE;
   }
+  const bool det = deterministic();
+  if (det && d_latent && !latent_scatter_fixed) {
+    set_error("deterministic mode is not available in this build");
+    return PNR_ERR_UNSUPPORTED;
+  }
   const int64_t cp = chunk_points(sc, total_points);
   Arena ar(ws, ws_bytes);
   Bufs b;
-  carve(ar, b, sc, mlp, cp);
+  carve(ar, b, sc, mlp, cp, det);
+  SplitKScope splitk(b.splitk, b.splitk_bytes);
   const bool want_cam = cam && (cam->d_poses || cam->d_focal || cam->d_c);
   const int V = sc.SB * NS;
   if (want_cam) PNR_CUDA(cudaMemsetAsync(b.cam_acc, 0, (size_t)V * 16 * sizeof(float), s));
@@ -545,9 +575,10 @@ int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src
     BW(rowsum_acc(b.tA, Rp, d, const_cast<float*>(grad.lin_in_b), s));
     BW(gemm(dh, d, b.w_inT, nullptr, b.dfeat, 48, R, 48, d, false, false, s));
     float* cam_part = want_cam ? b.T : nullptr;    // [R][16]; T (R x d, d >= 16) is free again here
-    k_geom_bwd<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(sc, src, g0, n, b.dfeat, b.dlat, d_latent, d_xyz,
-                                                               d_dirs, cam_part);
+    k_geom_bwd<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(sc, src, g0, n, b.dfeat, b.dlat,
+                                                               det ? nullptr : d_latent, d_xyz, d_dirs, cam_part);
     PNR_LAUNCH_CHECK();
+    if (det && d_latent) BW(latent_scatter_fixed(sc, src, g0, n, b.dlat, d_latent, b.lat_fixed, b.m_bits, s));
     if (want_cam) {
       k_cam_reduce<<<V, kCamThreads, 0, s>>>(cam_part, g0, n, src.P, NS, b.cam_acc);
       PNR_LAUNCH_CHECK();

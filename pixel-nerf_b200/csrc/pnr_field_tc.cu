@@ -1021,6 +1021,10 @@ int pnr_project_latent(const PnrScene* sc, const PnrMlp* mlp, float* proj, size_
   cudaStream_t s = (cudaStream_t)stream;
   float* bias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
   const int64_t rows = (int64_t)sc->SB * sc->NS * sc->Hl * sc->Wl;
+  // deterministic mode: the rest of the workspace holds the GEMM's split-K partials
+  const size_t used = (size_t)((reinterpret_cast<char*>(bias + 3 * tc::D) - static_cast<char*>(workspace)) + 255) & ~(size_t)255;
+  SplitKScope splitk(reinterpret_cast<float*>(static_cast<char*>(workspace) + used),
+                     workspace_bytes > used ? workspace_bytes - used : 0);
   for (int i = 0; i < 3; ++i) {
     const float* extra = (i == 0) ? mlp->lin_in_b : mlp->fc1_b[i - 1];
     tc::k_proj_bias<<<2, 256, 0, s>>>(mlp->lin_z_b[i], extra, bias + i * tc::D, tc::D);

@@ -14,7 +14,8 @@
 //              128B-swizzled tiles (the layout pnr_field_tc.cu uses), 3-stage ring
 //   MMA      : each warpgroup issues 12 wgmma per 64-wide k-step for its 64 rows and keeps one k-step in flight
 //              while the next one is loaded
-//   epilogue : registers -> (+ bias) -> store / read-add-store / red.global.add (split-K)
+//   epilogue : registers -> (+ bias) -> store / read-add-store / red.global.add (split-K); in deterministic mode a
+//              split stores its partial tile and k_splitk_sum adds the partials in split order
 // Roofline: tensor-bound for large K, but both operands arrive as fp32 through L2 (8 B per bf16-pair element), so
 // the practical bound is L2->SM bandwidth: 64 KB of operands per 1 M MAC k-step.
 #include <cuda_bf16.h>
@@ -44,8 +45,9 @@ struct Params {
   float* C;
   int lda, ldw, ldc, M, N, K;
   int k_per_split;   // multiple of BK
-  int relu_a, mode;  // mode 0: store, 1: C += (single split), 2: atomic add (split-K)
+  int relu_a, mode;  // mode 0: store, 1: C += (single split), 2: atomic add (split-K), 3: store into part (split-K)
   const float* mask; // optional [M][ldc]: the product is zeroed where mask <= 0 (ReLU backward) before store / add
+  float* part;       // mode 3: [splits][M][N] partial tiles
 };
 
 // 8 fp32 values -> error-compensated 16-bit pairs x = hi + lo.  BF16: 8 + 8 mantissa bits with fp32's exponent range
@@ -171,11 +173,28 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_gemm_split3(const __grid_consta
     float o = acc[i];
     if (p.mask && !(p.mask[(size_t)m * p.ldc + n] > 0.f)) o = 0.f;
     if (add_bias) o += __ldg(p.bias + n);
+    if (p.mode == 3) {
+      p.part[((size_t)blockIdx.z * p.M + m) * p.N + n] = o;
+      continue;
+    }
     float* dst = p.C + (size_t)m * p.ldc + n;
     if (p.mode == 2) atomicAdd(dst, o);
     else if (p.mode == 1) *dst += o;
     else *dst = o;
   }
+}
+
+// C (+)= ((P0 + P1) + P2) + ...: the partial tiles of an ordered split-K, summed in split order
+__global__ void k_splitk_sum(const float* __restrict__ part, int splits, int M, int N, float* __restrict__ C, int ldc,
+                             int accum) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t mn = (int64_t)M * N;
+  if (i >= mn) return;
+  float s = part[i];
+  for (int z = 1; z < splits; ++z) s += part[z * mn + i];
+  float* dst = C + (i / N) * ldc + i % N;
+  if (accum) *dst += s;
+  else *dst = s;
 }
 
 }  // namespace gemmtc
@@ -209,11 +228,19 @@ static int gemm_split3(bool bf16, const float* A, int lda, const float* W, int l
     if (splits > ksteps / 4) splits = ksteps / 4;
     if (splits < 1) splits = 1;
   }
+  // deterministic mode: the partials go to the installed scratch and are summed in order; never more splits than it
+  // holds (none installed: no split)
+  const bool ordered = splits > 1 && deterministic();
+  if (ordered) {
+    const size_t fit = splitk_scratch().bytes / ((size_t)M * N * sizeof(float));
+    if ((size_t)splits > fit) splits = fit > 1 ? (int)fit : 1;
+  }
   const int steps_per = (ksteps + splits - 1) / splits;
   splits = (ksteps + steps_per - 1) / steps_per;
   p.k_per_split = steps_per * BK;
-  p.mode = splits > 1 ? 2 : (accum ? 1 : 0);
-  if (splits > 1 && !accum) PNR_CUDA(cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, s));
+  p.mode = splits > 1 ? (ordered ? 3 : 2) : (accum ? 1 : 0);
+  p.part = p.mode == 3 ? splitk_scratch().p : nullptr;
+  if (p.mode == 2 && !accum) PNR_CUDA(cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, s));
   static bool attr_set[64] = {false};
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
     PNR_CUDA(cudaFuncSetAttribute(k_gemm_split3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
@@ -226,6 +253,11 @@ static int gemm_split3(bool bf16, const float* A, int lda, const float* W, int l
   else k_gemm_split3<false><<<grid, NTHREADS, SMEM_BYTES, s>>>(p);
   prof_after(s);
   PNR_LAUNCH_CHECK();
+  if (p.mode == 3) {
+    const int64_t mn = (int64_t)M * N;
+    k_splitk_sum<<<(unsigned)((mn + 255) / 256), 256, 0, s>>>(p.part, splits, M, N, C, ldc, accum ? 1 : 0);
+    PNR_LAUNCH_CHECK();
+  }
   return PNR_OK;
 }
 

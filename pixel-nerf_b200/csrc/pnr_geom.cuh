@@ -75,6 +75,53 @@ __device__ __forceinline__ PointGeom point_geometry(const PnrScene& sc, int sb, 
   return g;
 }
 
+// The bilinear taps of point x in view v of object sb as k_geom_bwd (pnr_field_bwd.cu) computes them, with the
+// backward's contractible arithmetic rather than point_geometry's; the fixed-point latent scatter of pnr_determ.cu
+// uses them.  k_geom_bwd keeps its own inline copy, so the default path's code is unchanged.
+struct BwdTaps {
+  bool vx1, vy1;                   // the second tap of x / y lies inside the map (taps outside carry nothing)
+  float w_nw, w_ne, w_sw, w_se;
+  size_t o_nw, o_ne, o_sw, o_se;   // channels-last offsets of the four taps into the latent
+};
+
+__device__ __forceinline__ BwdTaps bwd_taps(const PnrScene& sc, int sb, int v, const float x[3]) {
+  const float* M = sc.poses + (size_t)(sb * sc.NS + v) * 12;
+  float q[3], p[3];
+  for (int i = 0; i < 3; ++i) {
+    q[i] = M[i * 4 + 0] * x[0] + M[i * 4 + 1] * x[1] + M[i * 4 + 2] * x[2];
+    p[i] = q[i] + M[i * 4 + 3];
+  }
+  const float* fo = sc.focal + (sc.n_focal > 1 ? sb * 2 : 0);
+  const float* cc = sc.c + (sc.n_c > 1 ? sb * 2 : 0);
+  const float u = (-p[0] / p[2]) * fo[0] + cc[0];
+  const float w = (-p[1] / p[2]) * fo[1] + cc[1];
+  const int C = sc.C, Wl = sc.Wl, Hl = sc.Hl;
+  const float kx = sc.scale_x / sc.image_w, ky = sc.scale_y / sc.image_h;
+  const float ix_u = ((u * kx - 1.0f) + 1.0f) * 0.5f * (float)(Wl - 1);
+  const float iy_u = ((w * ky - 1.0f) + 1.0f) * 0.5f * (float)(Hl - 1);
+  float ix = fminf((float)(Wl - 1), fmaxf(ix_u, 0.f));
+  float iy = fminf((float)(Hl - 1), fmaxf(iy_u, 0.f));
+  if (!(ix == ix)) ix = 0.f;
+  if (!(iy == iy)) iy = 0.f;
+  const float x0f = floorf(ix), y0f = floorf(iy);
+  const int x0 = (int)x0f, y0 = (int)y0f;
+  BwdTaps t;
+  t.vx1 = (x0 + 1 <= Wl - 1);
+  t.vy1 = (y0 + 1 <= Hl - 1);
+  const int x1 = t.vx1 ? x0 + 1 : x0, y1 = t.vy1 ? y0 + 1 : y0;
+  const float wx0 = (x0f + 1.0f) - ix, wx1 = ix - x0f, wy0 = (y0f + 1.0f) - iy, wy1 = iy - y0f;
+  const size_t vbase = (size_t)(sb * sc.NS + v) * Hl * Wl * C;
+  t.o_nw = vbase + ((size_t)y0 * Wl + x0) * C;
+  t.o_ne = vbase + ((size_t)y0 * Wl + x1) * C;
+  t.o_sw = vbase + ((size_t)y1 * Wl + x0) * C;
+  t.o_se = vbase + ((size_t)y1 * Wl + x1) * C;
+  t.w_nw = wx0 * wy0;
+  t.w_ne = t.vx1 ? wx1 * wy0 : 0.f;
+  t.w_sw = t.vy1 ? wx0 * wy1 : 0.f;
+  t.w_se = (t.vx1 && t.vy1) ? wx1 * wy1 : 0.f;
+  return t;
+}
+
 __device__ __forceinline__ float feat_channel(const PointGeom& g, int ch) {
   // [q(3) | for k<6: sin(q f_k)(3), sin(q f_k + pi/2)(3) | R dir (3)], f_k = 1.5 * 2^k
   if (ch < 3) return g.q[ch];

@@ -7,7 +7,24 @@ import torch.nn.functional as F
 import torchvision
 from torch import nn
 
+import pnr_native as pn
 import util
+
+
+class _UpsampleAC(torch.autograd.Function):
+    """F.interpolate(x, size, mode="bilinear", align_corners=True) whose backward is pnr_upsample_bilinear_ac_backward,
+    a gather in a fixed order: torch's CUDA backward adds with atomics and raises under
+    torch.use_deterministic_algorithms(True).  The forward is torch's own call, so its output has the same bits."""
+
+    @staticmethod
+    def forward(ctx, x, size):
+        ctx.in_hw = x.shape[-2:]
+        ctx.dtype = x.dtype
+        return F.interpolate(x, size, mode="bilinear", align_corners=True)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        return pn.upsample_bilinear_ac_backward(d_out, ctx.in_hw).to(ctx.dtype), None
 
 
 class SpatialEncoder(nn.Module):
@@ -64,7 +81,9 @@ class SpatialEncoder(nn.Module):
             x = stage(x)
             maps.append(x)
         size = maps[0].shape[-2:]
-        maps = [F.interpolate(t, size, mode=self.upsample_interp, align_corners=True) for t in maps]
+        det = torch.are_deterministic_algorithms_enabled() and self.upsample_interp == "bilinear"
+        maps = [_UpsampleAC.apply(t, size) if (det and t.is_cuda and t.requires_grad)
+                else F.interpolate(t, size, mode=self.upsample_interp, align_corners=True) for t in maps]
         self.latents = maps
         self.latent = torch.cat(maps, dim=1)
         self.latent_scaling[0] = self.latent.shape[-1]

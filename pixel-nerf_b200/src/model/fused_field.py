@@ -49,6 +49,7 @@ class _FusedField(torch.autograd.Function):
         d_dirs = torch.empty(SB, B, 3, dtype=torch.float32, device=dev) if ctx.needs_input_grad[3] else None
         cam, d_cam = pn.camera_grad(net, ctx.needs_input_grad[5:8], dev)
         L = pn.lib()
+        pn.sync_deterministic()
         nbytes = L.pnr_field_backward_workspace_bytes(scene, m, B)
         ws = pn.workspace(dev, nbytes)
         with torch.cuda.device(dev):

@@ -208,7 +208,8 @@ class PixelNeRFNet(torch.nn.Module):
         return scene, mc, mf, keep
 
     def _projection(self, name, mstruct, nhwc, SB, NS):
-        key = (self._fused.latent_key, self._fused.mlp[name][0])
+        det = pn.sync_deterministic()          # the projection's split-K partials are summed in order when on
+        key = (self._fused.latent_key, self._fused.mlp[name][0], det)
         hit = self._fused.proj.get(name)
         if hit is not None and hit[0] == key:
             return hit[1]

@@ -161,6 +161,12 @@ def declare(L):
         L.pnr_mc_emit.argtypes = [vp, i32, i32, i32, f64, vp, vp, i64, i64, vp, sz, vp]
         for name in ("pnr_grid_points", "pnr_mc_count", "pnr_mc_emit"):
             getattr(L, name).restype = C.c_int
+    L.pnr_set_deterministic.argtypes = [C.c_int]
+    L.pnr_set_deterministic.restype = C.c_int
+    L.pnr_get_deterministic.restype = C.c_int
+    if hasattr(L, "pnr_upsample_bilinear_ac_backward"):   # (not in the host-emulator build of tests/cuda_emu)
+        L.pnr_upsample_bilinear_ac_backward.argtypes = [vp, i64, i32, i32, i32, i32, i32, vp, vp]
+        L.pnr_upsample_bilinear_ac_backward.restype = C.c_int
     L.pnr_gemm_nt.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]
     L.pnr_gemm_nt.restype = C.c_int
     L.pnr_profile_begin.restype = C.c_int
@@ -194,6 +200,27 @@ def lib():
 def check(rc):
     if rc != 0:
         raise RuntimeError(f"libpnr_sm90 error {rc}: {lib().pnr_last_error().decode()}")
+
+
+def sync_deterministic():
+    """Sets the library's deterministic-mode flag of the calling thread from torch.are_deterministic_algorithms_enabled()
+    (warn_only counts as on) and returns it.  Call it in the thread that makes the library call, before its workspace
+    query: the flag is thread-local and autograd runs backward on its own thread."""
+    on = torch.are_deterministic_algorithms_enabled()
+    lib().pnr_set_deterministic(1 if on else 0)
+    return on
+
+
+def upsample_bilinear_ac_backward(d_out, in_hw):
+    """pnr_upsample_bilinear_ac_backward: gradient [N][C][h_in][w_in] of F.interpolate(x, d_out's size,
+    mode="bilinear", align_corners=True) from d_out, in a fixed summation order."""
+    d_out = d_out.to(torch.float32).contiguous()
+    N, Cc, h_out, w_out = d_out.shape
+    d_in = torch.empty(N, Cc, int(in_hw[0]), int(in_hw[1]), dtype=torch.float32, device=d_out.device)
+    with torch.cuda.device(d_out.device):
+        check(lib().pnr_upsample_bilinear_ac_backward(dptr(d_out, "d_out"), N, Cc, d_in.shape[2], d_in.shape[3], h_out,
+                                                      w_out, dptr(d_in), stream_ptr(d_out.device)))
+    return d_in
 
 
 def dptr(t, name="tensor"):

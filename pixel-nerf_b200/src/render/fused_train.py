@@ -117,6 +117,7 @@ class _FusedRender(torch.autograd.Function):
             setattr(ug, name, pn.dptr(t, name))
         d_rays = torch.empty(SB, B, 8, dtype=torch.float32, device=dev) if ctx.needs_input_grad[4] else None
         cam, d_cam = pn.camera_grad(model, ctx.needs_input_grad[6:9], dev)
+        pn.sync_deterministic()
         nbytes = L.pnr_render_backward_workspace_bytes(scene, mc, mf, cfg, B)
         ws = pn.workspace(dev, nbytes)
         gfine = gstructs[1] if len(gstructs) > 1 else None
@@ -321,6 +322,7 @@ class _ShardedFusedRender(torch.autograd.Function):
         keep = [up, flat0]
         h = sharded._mgpu()
         ws_bytes = {}
+        pn.sync_deterministic()
         for i, (a, b) in enumerate(ctx.bounds):      # one workspace per device, sized for its largest shard
             if b - a > 0:
                 sh = ctx.shards[i]

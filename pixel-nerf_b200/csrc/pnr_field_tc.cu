@@ -20,10 +20,11 @@
 //  * lin_z[i](latent) is NOT a per-sample GEMM: bilinear interpolation commutes with a linear
 //    layer, so pnr_project_latent builds P_i = lin_z[i](latent) (+ biases) once per encode()
 //    and the epilogue gathers 4 taps of P_i and adds them to the residual stream.
-//  * Warp roles: 8 consumer warps (two warpgroups: geometry, wgmma, epilogues, ray finishing) and 1 weight-stream
-//    warp (cp.async.bulk of pre-swizzled 16 KB weight tiles in consumption order, 4-slot ring, mbarrier full/empty).
-//    ptxas allocates registers for 384 threads (168 per thread), so the 160 accumulator registers spill part of the
-//    epilogue state and serialize some wgmma: the kernel is correct, not yet tuned.
+//  * 256 threads = two warpgroups (geometry, wgmma, epilogues, ray finishing), so ptxas may give each thread 255
+//    registers: the 160 accumulator registers plus addressing fit, and each step's 9 or 12 wgmma issue back to back
+//    as one commit group.  There is no weight-stream warp: thread 0 refills the 4-slot ring (cp.async.bulk of
+//    pre-swizzled 16 KB weight tiles in consumption order, mbarrier full/empty) whenever a step's slots are released
+//    (struct Ring).  tests/test_tc_codegen.py guards the register budget.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
@@ -46,7 +47,7 @@ constexpr int ROWS = 64;                 // rows (points) per CTA
 constexpr int TILE_POINTS = 128;         // per tile index (two CTAs)
 constexpr int NCONSUMER_WARPS = 8;       // two warpgroups
 constexpr int NCONSUMERS = NCONSUMER_WARPS * 32;
-constexpr int NTHREADS = NCONSUMERS + 32;  // + warp 8: weight streamer
+constexpr int NTHREADS = NCONSUMERS;     // thread 0 also issues the weight-slot loads (no dedicated streamer warp)
 constexpr int SLOT_BYTES = 16384;        // 128 weight rows x 64 k x fp16
 constexpr int NSLOTS = 4;
 constexpr int A_CHUNK_BYTES = 16384;     // 64 rows x 64 k x fp16, hi then lo
@@ -68,7 +69,8 @@ constexpr int BAR_FULL = 0;                             // [NSLOTS]
 constexpr int BAR_EMPTY = BAR_FULL + NSLOTS;            // [NSLOTS]
 constexpr int BAR_COUNT = BAR_EMPTY + NSLOTS;
 constexpr int SM_NLIST = SM_BAR + BAR_COUNT * 8;        // fused render: number of rays this CTA completed in the current pass
-constexpr int SMEM_BYTES = SM_NLIST + 16;
+constexpr int SM_FEED = SM_NLIST + 16;                  // struct Feed: the weight-slot cursor of the producer thread
+constexpr int SMEM_BYTES = SM_FEED + 128;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
 constexpr int FLUSH_SCRATCH_BYTES = A_BYTES / NCONSUMER_WARPS;   // per-warp scratch (cdf + merged samples) in the idle A buffer
 
@@ -145,9 +147,62 @@ __device__ __forceinline__ uint32_t swz(int m, int k) {
   return (uint32_t)(m * 128 + ((((k >> 3) ^ (m & 7))) << 4) + (k & 7) * 2);
 }
 
-// Weight ring: the streamer fills the slots in exactly the order the consumers use them, and every step of a
-// consumer warpgroup takes two consecutive slots (W_hi, W_lo of one 128-row x 64-k tile).  A step's slots are
-// released once the wgmma that read them has completed (one step later: wait_group 1).
+extern __shared__ __align__(1024) uint8_t smem[];
+
+// The weight-slot sequence of one CTA, in consumption order: per pass, per tile of its pair, NS x (lin_in + blocks
+// 0-2: slots [0, 392) of the pass's weight image) then blocks 3-4 (slots [392, 648)).  Thread 0 walks it one slot at a
+// time; the cursor lives in shared memory so that no register is held for it across the MMA loops.
+struct Feed {
+  const uint8_t* slots[2];   // first slot of each pass's weight image
+  int64_t n_tiles[2];
+  int64_t tile;              // tile of the next slot
+  int npass, NS, pair, n_pairs;
+  int ps, v, i;              // pass (npass: sequence done), view (NS: the blocks 3-4 run), slot within the run
+  __device__ __forceinline__ void skip_empty_passes() {
+    while (ps < npass && tile >= n_tiles[ps]) {
+      ++ps;
+      tile = pair;
+    }
+  }
+};
+static_assert(sizeof(Feed) <= SMEM_BYTES - SM_FEED, "Feed does not fit its shared-memory slot");
+__device__ __forceinline__ Feed& feed() { return *reinterpret_cast<Feed*>(smem + SM_FEED); }
+
+// Producer (thread 0 only): load the two slots of the step whose first slot has sequence number n, once the slots'
+// previous contents (sequence numbers n - 4, n - 3) are released by all 8 warps.
+__device__ __forceinline__ void feed_step(uint32_t bar_base, uint32_t b_base, uint32_t n, int* status) {
+  Feed& f = feed();
+#pragma unroll 1
+  for (uint32_t s = n; s < n + 2; ++s) {
+    if (f.ps >= f.npass) return;
+    const uint32_t sl = s % NSLOTS, ph = (s / NSLOTS) & 1;
+    mbar_wait(bar_base + (BAR_EMPTY + sl) * 8, ph ^ 1, status, 400 + sl);
+    const uint32_t full = bar_base + (BAR_FULL + sl) * 8;
+    const bool head = f.v < f.NS;   // lin_in + blocks 0-2 of view v, else blocks 3-4
+    mbar_expect_tx(full, SLOT_BYTES);
+    bulk_g2s(b_base + sl * SLOT_BYTES,
+             f.slots[f.ps] + (size_t)((head ? 0 : SLOTS_LIN_IN + 3 * SLOTS_BLOCK) + f.i) * SLOT_BYTES, SLOT_BYTES, full);
+    if (++f.i == (head ? SLOTS_LIN_IN + 3 * SLOTS_BLOCK : 2 * SLOTS_BLOCK)) {
+      f.i = 0;
+      if (++f.v > f.NS) {
+        f.v = 0;
+        f.tile += f.n_pairs;
+        f.skip_empty_passes();
+      }
+    }
+  }
+}
+
+// Weight ring: 4 slots, filled in exactly the order the consumers use them; every step of a consumer warpgroup takes
+// two consecutive slots (W_hi, W_lo of one 128-row x 64-k tile).  A step's slots are released once the wgmma that read
+// them has completed (one step later: wait_group 1, or at the drain that ends an MMA run), and the release refills
+// them with the step two ahead: thread 0 waits until all 8 warps have released them (EMPTY), then issues the
+// cp.async.bulk.  Steps 0 and 1 are loaded at kernel start.
+// This EMPTY wait cannot deadlock: when thread 0 waits in the release of step s, warpgroup 1 still has to release s,
+// which it does in its own `issued` of step s+1 or its drain after step s, with no workers_sync in between (both
+// warpgroups run the same step sequence and every MMA run ends with a drain before the next workers_sync).  To get
+// there it needs only FULL of step s+1, and that load was issued at the release of step s-1, earlier in program order
+// of thread 0.  Warps 1-3 of warpgroup 0 arrive before they reach the next wgmma, so they do not wait on warp 0.
 struct Ring {
   uint32_t bar_base, b_base;
   uint32_t seq;      // slot sequence number of the next step
@@ -165,7 +220,9 @@ struct Ring {
     if (lane == 0) {
       mbar_arrive(bar_base + (BAR_EMPTY + s % NSLOTS) * 8);
       mbar_arrive(bar_base + (BAR_EMPTY + (s + 1) % NSLOTS) * 8);
+      if (threadIdx.x == 0) feed_step(bar_base, b_base, s + NSLOTS, status);
     }
+    __syncwarp();
   }
   // after the step's wgmma are issued: commit them as one group, retire the previous step
   __device__ __forceinline__ void issued() {
@@ -202,6 +259,30 @@ struct Cons {
   float w_scale, w_inv;
   uint64_t l2_keep;     // createpolicy evict_last (view-sum scratch)
 };
+
+// The epilogues address ~64 loop-invariant locations per thread (operand pairs, biases, scratch lines).  Left to
+// itself the compiler hoists all of them out of the tile loop and spills them; instead every epilogue call rebuilds
+// one base per buffer behind an opaque move and reaches the individual elements with immediate offsets.
+template <typename T>
+__device__ __forceinline__ T* opaque(T* v) {
+  asm volatile("" : "+l"(v));
+  return v;
+}
+__device__ __forceinline__ uint32_t opaque(uint32_t v) {
+  asm volatile("" : "+r"(v));
+  return v;
+}
+// Shared-memory address of the thread's accumulator pair (i, i + 1) of N block q in a buffer of 128B-swizzled
+// 64-wide k-chunks (A operand layout): swz(m, k) at m = r0 + 8 ((i >> 1) & 1), k = 8 (i >> 2) + c0 of chunk
+// 2 q + wg.  swz only XORs the 16-byte unit index (address bits 4-6) with m & 7 = r0 & 7, and every other term is a
+// multiple of 128 (the buffers are 1024-byte aligned) or below 16, so the XOR can be applied to the thread's base
+// swz(r0, c0) of chunk wg.
+__device__ __forceinline__ uint32_t acc_base(const Cons& c, uint32_t buf) {
+  return opaque(c.smem_u + buf + c.wg * A_CHUNK_BYTES + swz(c.r0, c.c0));
+}
+__device__ __forceinline__ uint32_t acc_addr(uint32_t base, int q, int i) {
+  return (base ^ (uint32_t)((i >> 2) << 4)) + q * 2 * A_CHUNK_BYTES + ((i >> 1) & 1) * 1024;
+}
 
 // lin_in (K = 42 -> 48) and the fc_1 steps over one 64-wide k-chunk: 4 steps of 128 output rows (N block q);
 // warpgroup g accumulates rows [64g, 64g+64) of each into x[q].
@@ -243,14 +324,14 @@ __device__ __forceinline__ void fc_block(Ring& rg, const Cons& c, float (&x)[4][
     fence_acc<32>(h);
     workers_sync();   // both warpgroups are done with relu(H_{c-1})
     // ---- relu(H_c + b0) -> fp16 hi/lo chunk g of the relu(H) buffer ----
-    const float* bc = b0 + hc * 128 + c.wg * 64;
+    const float* bc = opaque(b0 + hc * 128 + c.wg * 64 + c.c0);
+    const uint32_t ah = acc_base(c, SM_AH);
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
-      const int col = 8 * (i >> 2) + c.c0, m = c.r0 + 8 * ((i >> 1) & 1);
-      const float2 bb = __ldg(reinterpret_cast<const float2*>(bc + col));
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(bc + 8 * (i >> 2)));
       uint32_t hi, lo;
       split_relu2(h[i] * c.w_inv + bb.x, h[i + 1] * c.w_inv + bb.y, hi, lo);
-      const uint32_t a = c.smem_u + SM_AH + c.wg * A_CHUNK_BYTES + swz(m, col);
+      const uint32_t a = acc_addr(ah, 0, i);
       st_shared_u32(a, hi);
       st_shared_u32(a + 8192, lo);
     }
@@ -321,24 +402,29 @@ __device__ __forceinline__ void epilogue_x(Ring& rg, const Cons& c, float (&x)[4
     workers_sync();
   }
   float o[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+  // feature f = 128 q + 64 wg + 8 (i >> 2) + c0 of row m = r0 + 8 ((i >> 1) & 1)
+  const uint32_t xa = acc_base(c, SM_A);
+  // the staged G pair of (m, f, f + 1) sits in the hi (c0 < 4) or lo unit of 8-feature group f & ~7 (stage_gather)
+  const uint32_t ga = opaque(c.smem_u + SM_A + c.wg * A_CHUNK_BYTES + swz(c.r0, 0) + (c.c0 >= 4 ? 8192u : 0u) +
+                             (c.c0 & 3) * 4);
+  const float* bp = MODE == MODE_GATHER ? nullptr : opaque(bias + 64 * c.wg + c.c0);
+  const float* wp = MODE == MODE_OUT ? opaque(lin_out_w + 64 * c.wg + c.c0) : nullptr;
+  float* sp0 = MODE == MODE_COMBINE ? opaque(scratch + c.tid) : nullptr;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
-      const int r = (i >> 1) & 1, m = c.r0 + 8 * r;
-      const int f = 128 * q + 64 * c.wg + 8 * (i >> 2) + c.c0;
+      const int r = (i >> 1) & 1;
       float y0 = x[q][i] * c.w_inv, y1 = x[q][i + 1] * c.w_inv;
       if (MODE == MODE_GATHER) {
-        // the staged G pair of (m, f, f+1); the quad that shares its 16-byte units reads them all before any writes
-        const uint32_t a = c.smem_u + SM_A + (f >> 6) * A_CHUNK_BYTES + swz(m, (f & 63) & ~7) + (c.c0 >= 4 ? 8192u : 0u) +
-                           (c.c0 & 3) * 4;
+        // the quad that shares the G pair's 16-byte units reads them all before any writes
         float2 g;
-        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(g.x), "=f"(g.y) : "r"(a) : "memory");
+        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(g.x), "=f"(g.y) : "r"(acc_addr(ga, q, i)) : "memory");
         __syncwarp();
         y0 += g.x;
         y1 += g.y;
       } else {
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + f));
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bp + 128 * q + 8 * (i >> 2)));
         y0 += bb.x;
         y1 += bb.y;
       }
@@ -346,7 +432,7 @@ __device__ __forceinline__ void epilogue_x(Ring& rg, const Cons& c, float (&x)[4
         // view-sum scratch (thread-private, coalesced): 128 KB per CTA that every CTA rewrites and re-reads NS-1
         // times per tile.  With both MLPs' projected maps and weight images streaming through the 50 MB L2, plain
         // LRU would evict DIRTY scratch lines to DRAM; evict_last keeps the small hot scratch resident instead
-        float* sp = scratch + (size_t)((q * 32 + i) * NCONSUMERS + c.tid);
+        float* sp = sp0 + (q * 32 + i) * NCONSUMERS;
         if (view == 0) {
           st_evict_last(sp, y0, c.l2_keep);
           st_evict_last(sp + NCONSUMERS, y1, c.l2_keep);
@@ -367,7 +453,7 @@ __device__ __forceinline__ void epilogue_x(Ring& rg, const Cons& c, float (&x)[4
         const float a0 = fmaxf(y0, 0.f), a1 = fmaxf(y1, 0.f);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          const float2 w = __ldg(reinterpret_cast<const float2*>(lin_out_w + k * D + f));
+          const float2 w = __ldg(reinterpret_cast<const float2*>(wp + k * D + 128 * q + 8 * (i >> 2)));
           o[r][k] = fmaf(a1, w.y, fmaf(a0, w.x, o[r][k]));
         }
       } else if (produce) {
@@ -375,7 +461,7 @@ __device__ __forceinline__ void epilogue_x(Ring& rg, const Cons& c, float (&x)[4
         x[q][i + 1] = y1 * c.w_scale;
         uint32_t hi, lo;
         split_relu2(y0, y1, hi, lo);
-        const uint32_t a = c.smem_u + SM_A + (f >> 6) * A_CHUNK_BYTES + swz(m, f & 63);
+        const uint32_t a = acc_addr(xa, q, i);
         st_shared_u32(a, hi);
         st_shared_u32(a + 8192, lo);
       }
@@ -460,7 +546,6 @@ __device__ __forceinline__ void finish_ray(const Params& p, int ps, int64_t ray,
 }
 
 __global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant__ Params p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = blockIdx.x & 1;        // which 64 points of the 128-point tile
   const int pair = blockIdx.x >> 1;
@@ -476,13 +561,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant_
       mbar_init(bar_base + (BAR_EMPTY + i) * 8, NCONSUMER_WARPS);
     }
     *n_list = 0;
+    Feed& f = feed();
+    for (int i = 0; i < 2; ++i) {
+      f.slots[i] = i < p.npass ? p.pass[i].packed + HEADER_BYTES : nullptr;
+      f.n_tiles[i] = i < p.npass ? p.pass[i].n_tiles : 0;
+    }
+    f.npass = p.npass;
+    f.NS = NS;
+    f.pair = pair;
+    f.n_pairs = n_pairs;
+    f.ps = 0;
+    f.v = 0;
+    f.i = 0;
+    f.tile = pair;
+    f.skip_empty_passes();
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  if (threadIdx.x == 0) {
+    // prefill: steps 0 and 1 (the EMPTY waits of the first use of a slot return at once)
+    feed_step(bar_base, smem_u32(smem + SM_B), 0, p.status);
+    feed_step(bar_base, smem_u32(smem + SM_B), 2, p.status);
+  }
   const size_t map_stride = (size_t)p.sc.SB * NS * p.sc.Hl * p.sc.Wl * D;
 
-  if (warp < NCONSUMER_WARPS) {
-    // =============================== consumer warpgroups ===============================
+  {
     Cons c;
     c.smem_u = smem_u32(smem);
     c.tid = threadIdx.x;
@@ -663,29 +766,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant_
         workers_sync();
         if (threadIdx.x == 0) *n_list = 0;
         // (the next pass's first write to n_list happens after several workers_sync of its first tile)
-      }
-    }
-  } else if (lane == 0) {
-    // =============================== weight streamer ===============================
-    uint32_t seq = 0;
-    const uint32_t b_base = smem_u32(smem + SM_B);
-    const uint8_t* slots = nullptr;
-    auto stream = [&](int first, int count) {
-      for (int i = first; i < first + count; ++i) {
-        const uint32_t sl = seq % NSLOTS, ph = (seq / NSLOTS) & 1;
-        mbar_wait(bar_base + (BAR_EMPTY + sl) * 8, ph ^ 1, p.status, 400 + sl);
-        const uint32_t full = bar_base + (BAR_FULL + sl) * 8;
-        mbar_expect_tx(full, SLOT_BYTES);
-        bulk_g2s(b_base + sl * SLOT_BYTES, slots + (size_t)i * SLOT_BYTES, SLOT_BYTES, full);
-        ++seq;
-      }
-    };
-    for (int ps = 0; ps < p.npass; ++ps) {
-      slots = p.pass[ps].packed + HEADER_BYTES;
-      const int64_t n_tiles = p.pass[ps].n_tiles;
-      for (int64_t tile = pair; tile < n_tiles; tile += n_pairs) {
-        for (int v = 0; v < NS; ++v) stream(0, SLOTS_LIN_IN + 3 * SLOTS_BLOCK);
-        stream(SLOTS_LIN_IN + 3 * SLOTS_BLOCK, 2 * SLOTS_BLOCK);
       }
     }
   }

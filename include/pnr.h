@@ -41,7 +41,17 @@ enum {
 enum {
   PNR_ENGINE_AUTO = 0,   /* tensor engine when the shape allows it, else SIMT            */
   PNR_ENGINE_SIMT = 1,   /* fp32 FFMA kernels, any shape (bring-up / small-d engine)      */
-  PNR_ENGINE_TC = 2      /* wgmma split-fp16 (3 products, fp32 accumulate) fused kernel */
+  PNR_ENGINE_TC = 2,     /* wgmma split-fp16 (3 products, fp32 accumulate) fused kernel: rgb within 1e-4 of fp32 */
+  /* 3 is PNR_GEMM_F16X3 (pnr_gemm_nt only).
+   * Single-pass tensor engine, inference only: the same fused kernel with ONE fp16 product per GEMM
+   * (D += Ahi*Whi, fp32 accumulate) for lin_in, fc_0 and fc_1; lin_z, geometry, the view mean, lin_out, compositing and
+   * resampling stay as in PNR_ENGINE_TC.  Expect rgb errors against fp32 of a few 1e-4 on real scenes and up to
+   * about one uint8 step (a few 1e-3), and more importance-sampling bin flips; DESIGN.md 3.1 has the measured
+   * figures.  Never chosen by AUTO; the shape requirements of PNR_ENGINE_TC (PNR_ERR_UNSUPPORTED otherwise, no
+   * fallback).  The render backward entry points (pnr_render_backward*, pnr_mgpu_render_backward*) refuse it with
+   * PNR_ERR_INVALID: their recompute could not reproduce this forward.  pnr_field_backward* take no engine and
+   * always recompute on the exact arithmetic, so a caller must not pair them with a forward of this engine. */
+  PNR_ENGINE_TC_FAST = 4
 };
 
 /* State left behind by PixelNeRFNet.encode (src/model/models.py:89-144) and

@@ -80,16 +80,17 @@ static int check_mlp(const PnrMlp* m) {
   return PNR_OK;
 }
 
-// engine actually used for (scene, mlp): AUTO prefers the tensor engine when it applies.
+// engine actually used for (scene, mlp): AUTO prefers the tensor engine when it applies (never the single-pass one).
 static int resolve_engine(const PnrScene& sc, const PnrMlp& mlp, const float* proj, int engine) {
   bool tc_ok = tc_supported(sc, mlp) && mlp.packed != nullptr && proj != nullptr;
-  if (engine == PNR_ENGINE_TC) {
+  if (engine == PNR_ENGINE_TC || engine == PNR_ENGINE_TC_FAST) {
     if (!tc_ok) {
-      set_error("tensor engine unavailable for this call (needs d_hidden=512, d_latent=512, 5 blocks, "
-                "combine_layer=3, packed weights and projected latent)");
+      set_error("%s unavailable for this call (needs d_hidden=512, d_latent=512, 5 blocks, "
+                "combine_layer=3, packed weights and projected latent)",
+                engine == PNR_ENGINE_TC ? "tensor engine" : "single-pass tensor engine (PNR_ENGINE_TC_FAST)");
       return PNR_ERR_UNSUPPORTED;
     }
-    return PNR_ENGINE_TC;
+    return engine;
   }
   if (engine == PNR_ENGINE_SIMT) return PNR_ENGINE_SIMT;
   if (engine == PNR_ENGINE_AUTO) return tc_ok ? PNR_ENGINE_TC : PNR_ENGINE_SIMT;
@@ -101,7 +102,7 @@ static size_t field_ws(const PnrScene& sc, const PnrMlp& mlp, int64_t total_poin
   size_t a = simt_workspace_bytes(sc, mlp, total_points);
   if (engine == PNR_ENGINE_SIMT) return a;
   size_t b = tc_supported(sc, mlp) ? tc_workspace_bytes(sc, mlp, total_points) : 0;
-  if (engine == PNR_ENGINE_TC) return b;
+  if (engine == PNR_ENGINE_TC || engine == PNR_ENGINE_TC_FAST) return b;
   return a > b ? a : b;
 }
 
@@ -111,7 +112,19 @@ static int field_dispatch(const PnrScene& sc, const PnrMlp& mlp, const float* pr
   int e = resolve_engine(sc, mlp, proj, engine);
   if (e < 0) return e;
   if (e == PNR_ENGINE_TC) return tc_field_eval(sc, mlp, proj, src, total_points, out, ws, ws_bytes, s);
+  if (e == PNR_ENGINE_TC_FAST) return tc_field_eval_fast(sc, mlp, proj, src, total_points, out, ws, ws_bytes, s);
   return simt_field_eval(sc, mlp, src, total_points, out, ws, ws_bytes, s);
+}
+
+// The backward recomputes the forward's field values on the exact arithmetic, so it cannot differentiate what the
+// single-pass engine rendered; it refuses that engine instead of silently running another one.
+int check_backward_engine(int engine) {
+  if (engine == PNR_ENGINE_TC_FAST) {
+    set_error("PNR_ENGINE_TC_FAST is inference only: the backward cannot reproduce its forward (train with "
+              "PNR_ENGINE_TC or PNR_ENGINE_AUTO)");
+    return PNR_ERR_INVALID;
+  }
+  return PNR_OK;
 }
 
 }  // namespace pnr
@@ -336,7 +349,7 @@ static int check_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse
                     cfg->n_fine_depth <= cfg->n_fine,
                 "bad sample counts");
   PNR_CHECK_ARG(B >= 0, "B must be >= 0");
-  return PNR_OK;
+  return check_backward_engine(cfg->engine);
 }
 
 int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
@@ -537,7 +550,7 @@ int pnr_render(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* ml
     if (ec < 0) return ec;
     int ef = Kf > 0 ? resolve_engine(*scene, *mf, pf, cfg->engine) : ec;
     if (ef < 0) return ef;
-    if (ec == PNR_ENGINE_TC && ef == PNR_ENGINE_TC && fused_render_enabled())
+    if ((ec == PNR_ENGINE_TC || ec == PNR_ENGINE_TC_FAST) && ef == ec && fused_render_enabled())
       return tc_render(*scene, *mlp_coarse, *mf, scene->proj_coarse, pf, *cfg, rays, *noise, zc, wc, zf, *out, B, rest,
                        rest_bytes, s);
   }

@@ -133,6 +133,9 @@ int launch_ray_grad(const float* rays, const float* z, const float* d_z, const f
 int launch_gen_rays_bwd(const float* d_rays, int W, int H, float fx, float fy, float cx, float cy, int64_t first,
                         int64_t count, float* d_poses, cudaStream_t s);
 
+// PNR_ERR_INVALID (with the message) for an engine the backward entry points refuse: PNR_ENGINE_TC_FAST (pnr_api.cu)
+int check_backward_engine(int engine);
+
 // ---- field backward, SIMT first path (pnr_field_bwd.cu) --------------------------------
 size_t field_backward_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int64_t total_points);
 int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src, int64_t total_points,
@@ -144,8 +147,14 @@ bool tc_supported(const PnrScene& sc, const PnrMlp& mlp);
 size_t tc_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int64_t total_points);
 int tc_field_eval(const PnrScene& sc, const PnrMlp& mlp, const float* proj, const PointSource& src,
                   int64_t total_points, float* out, void* ws, size_t ws_bytes, cudaStream_t s);
+// tc_field_eval on the single-pass kernel (PNR_ENGINE_TC_FAST).  Weak: the host-emulator build has no tensor engine
+// (tc_supported is false there, so this is never reached) and still links without it.
+int tc_field_eval_fast(const PnrScene& sc, const PnrMlp& mlp, const float* proj, const PointSource& src,
+                       int64_t total_points, float* out, void* ws, size_t ws_bytes, cudaStream_t s)
+    __attribute__((weak));
 // NeRFRenderer.forward in one launch (coarse + fine field passes with compositing / resampling in the ray-completion
-// epilogue); zc, wc [R][Kc] and zf [R][Kc+Kf] are caller or workspace buffers that also serve as outputs.
+// epilogue); zc, wc [R][Kc] and zf [R][Kc+Kf] are caller or workspace buffers that also serve as outputs.  The kernel is
+// the single-pass one when cfg.engine is PNR_ENGINE_TC_FAST.
 size_t tc_render_workspace_bytes(const PnrScene& sc, int64_t R, int Kc, int Kf);
 int tc_render(const PnrScene& sc, const PnrMlp& mlp_coarse, const PnrMlp& mlp_fine, const float* proj_coarse,
               const float* proj_fine, const PnrRenderCfg& cfg, const float* rays, const PnrNoise& noise, float* zc,

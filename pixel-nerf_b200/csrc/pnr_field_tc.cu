@@ -25,6 +25,10 @@
 //    as one commit group.  There is no weight-stream warp: thread 0 refills the 4-slot ring (cp.async.bulk of
 //    pre-swizzled 16 KB weight tiles in consumption order, mbarrier full/empty) whenever a step's slots are released
 //    (struct Ring).  tests/test_tc_codegen.py guards the register budget.
+//  * k_field_tc_fast (PNR_ENGINE_TC_FAST) is the same body with FAST = true: one tensor pass per step, D += Ahi*Whi
+//    with fp32 accumulation.  It loads only the W_hi tile of each step (the W_lo slot of the ring stays idle) and never
+//    writes the fp16 lo halves of its A operands.  The projected-latent gather (lin_z stays exact), geometry, the view
+//    mean, lin_out, compositing, resampling and the flush are the same code.  tests/test_tc_fast_codegen.py.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
@@ -142,6 +146,12 @@ __device__ __forceinline__ void split_relu2(float y0, float y1, uint32_t& hi, ui
   const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(a1 - hf.y), "f"(a0 - hf.x));
 }
+// relu(y0), relu(y1) -> packed fp16 pair, the hi half of split_relu2 (single-pass engine)
+__device__ __forceinline__ uint32_t relu_f16x2(float y0, float y1) {
+  uint32_t hi;
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(fmaxf(y1, 0.f)), "f"(fmaxf(y0, 0.f)));
+  return hi;
+}
 // byte offset of the 16-bit pair (row m, k columns [k, k+2) of the 64-wide chunk), k even, in a 128B-swizzled tile
 __device__ __forceinline__ uint32_t swz(int m, int k) {
   return (uint32_t)(m * 128 + ((((k >> 3) ^ (m & 7))) << 4) + (k & 7) * 2);
@@ -169,19 +179,25 @@ static_assert(sizeof(Feed) <= SMEM_BYTES - SM_FEED, "Feed does not fit its share
 __device__ __forceinline__ Feed& feed() { return *reinterpret_cast<Feed*>(smem + SM_FEED); }
 
 // Producer (thread 0 only): load the two slots of the step whose first slot has sequence number n, once the slots'
-// previous contents (sequence numbers n - 4, n - 3) are released by all 8 warps.
+// previous contents (sequence numbers n - 4, n - 3) are released by all 8 warps.  The single-pass engine loads the
+// W_hi slot only (even sequence numbers: the weight image stores every tile as hi, lo) and steps the cursor over W_lo.
+template <bool FAST>
 __device__ __forceinline__ void feed_step(uint32_t bar_base, uint32_t b_base, uint32_t n, int* status) {
   Feed& f = feed();
 #pragma unroll 1
   for (uint32_t s = n; s < n + 2; ++s) {
     if (f.ps >= f.npass) return;
+    const bool load = !FAST || s % 2 == 0;
     const uint32_t sl = s % NSLOTS, ph = (s / NSLOTS) & 1;
-    mbar_wait(bar_base + (BAR_EMPTY + sl) * 8, ph ^ 1, status, 400 + sl);
+    if (load) mbar_wait(bar_base + (BAR_EMPTY + sl) * 8, ph ^ 1, status, 400 + sl);
     const uint32_t full = bar_base + (BAR_FULL + sl) * 8;
     const bool head = f.v < f.NS;   // lin_in + blocks 0-2 of view v, else blocks 3-4
-    mbar_expect_tx(full, SLOT_BYTES);
-    bulk_g2s(b_base + sl * SLOT_BYTES,
-             f.slots[f.ps] + (size_t)((head ? 0 : SLOTS_LIN_IN + 3 * SLOTS_BLOCK) + f.i) * SLOT_BYTES, SLOT_BYTES, full);
+    if (load) {
+      mbar_expect_tx(full, SLOT_BYTES);
+      bulk_g2s(b_base + sl * SLOT_BYTES,
+               f.slots[f.ps] + (size_t)((head ? 0 : SLOTS_LIN_IN + 3 * SLOTS_BLOCK) + f.i) * SLOT_BYTES, SLOT_BYTES,
+               full);
+    }
     if (++f.i == (head ? SLOTS_LIN_IN + 3 * SLOTS_BLOCK : 2 * SLOTS_BLOCK)) {
       f.i = 0;
       if (++f.v > f.NS) {
@@ -203,6 +219,9 @@ __device__ __forceinline__ void feed_step(uint32_t bar_base, uint32_t b_base, ui
 // warpgroups run the same step sequence and every MMA run ends with a drain before the next workers_sync).  To get
 // there it needs only FULL of step s+1, and that load was issued at the release of step s-1, earlier in program order
 // of thread 0.  Warps 1-3 of warpgroup 0 arrive before they reach the next wgmma, so they do not wait on warp 0.
+// FAST (single-pass engine): the same sequence numbers and the same protocol on each step's first (W_hi) slot only;
+// the barriers of the W_lo slots are never used.
+template <bool FAST>
 struct Ring {
   uint32_t bar_base, b_base;
   uint32_t seq;      // slot sequence number of the next step
@@ -212,15 +231,15 @@ struct Ring {
   int* status;
   __device__ __forceinline__ uint32_t slot_addr(uint32_t s) const { return b_base + (s % NSLOTS) * SLOT_BYTES; }
   __device__ __forceinline__ void acquire() {
-    for (uint32_t s = seq; s < seq + 2; ++s)
+    for (uint32_t s = seq; s < seq + (FAST ? 1 : 2); ++s)
       mbar_wait(bar_base + (BAR_FULL + s % NSLOTS) * 8, (s / NSLOTS) & 1, status, 200 + (int)(s % NSLOTS));
   }
   __device__ __forceinline__ void release(uint32_t s) {
     __syncwarp();
     if (lane == 0) {
       mbar_arrive(bar_base + (BAR_EMPTY + s % NSLOTS) * 8);
-      mbar_arrive(bar_base + (BAR_EMPTY + (s + 1) % NSLOTS) * 8);
-      if (threadIdx.x == 0) feed_step(bar_base, b_base, s + NSLOTS, status);
+      if (!FAST) mbar_arrive(bar_base + (BAR_EMPTY + (s + 1) % NSLOTS) * 8);
+      if (threadIdx.x == 0) feed_step<FAST>(bar_base, b_base, s + NSLOTS, status);
     }
     __syncwarp();
   }
@@ -240,13 +259,14 @@ struct Ring {
   }
 };
 
-// acc (+)= A[64 x 16 KSTEPS] * W^T over one step: Ahi*Whi + Alo*Whi + Ahi*Wlo
-template <int KSTEPS>
+// acc (+)= A[64 x 16 KSTEPS] * W^T over one step: Ahi*Whi + Alo*Whi + Ahi*Wlo (FAST: Ahi*Whi only)
+template <bool FAST, int KSTEPS>
 __device__ __forceinline__ void mma3(float* acc, uint64_t a_hi, uint64_t b_hi, uint64_t b_lo, bool zero) {
   const uint64_t a_lo = a_hi + (8192 >> 4);
 #pragma unroll
   for (int kk = 0; kk < KSTEPS; ++kk) {
     wgmma_m64n64_f16(acc, a_hi + 2 * kk, b_hi + 2 * kk, (zero && kk == 0) ? 0u : 1u);
+    if (FAST) continue;
     wgmma_m64n64_f16(acc, a_lo + 2 * kk, b_hi + 2 * kk, 1u);
     wgmma_m64n64_f16(acc, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
   }
@@ -286,8 +306,9 @@ __device__ __forceinline__ uint32_t acc_addr(uint32_t base, int q, int i) {
 
 // lin_in (K = 42 -> 48) and the fc_1 steps over one 64-wide k-chunk: 4 steps of 128 output rows (N block q);
 // warpgroup g accumulates rows [64g, 64g+64) of each into x[q].
-template <int KSTEPS>
-__device__ __forceinline__ void wide_steps(Ring& rg, const Cons& c, float (&x)[4][32], uint64_t a_hi, bool zero) {
+template <bool FAST, int KSTEPS>
+__device__ __forceinline__ void wide_steps(Ring<FAST>& rg, const Cons& c, float (&x)[4][32], uint64_t a_hi,
+                                           bool zero) {
   const uint64_t desc0 = make_desc(0);
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
@@ -296,14 +317,15 @@ __device__ __forceinline__ void wide_steps(Ring& rg, const Cons& c, float (&x)[4
     const uint64_t b_lo = desc0 + ((rg.slot_addr(rg.seq + 1) + c.wg * 8192) >> 4);
     fence_acc<32>(x[q]);
     wgmma_fence();
-    mma3<KSTEPS>(x[q], a_hi, b_hi, b_lo, zero);
+    mma3<FAST, KSTEPS>(x[q], a_hi, b_hi, b_lo, zero);
     rg.issued();
   }
 }
 
 // fc_0 and fc_1 of one ResNet block: X += W1 relu(W0 relu(X) + b0) (the fc_1 bias is added by the caller's epilogue).
-__device__ __forceinline__ void fc_block(Ring& rg, const Cons& c, float (&x)[4][32], const float* __restrict__ b0,
-                                         const int* status) {
+template <bool FAST>
+__device__ __forceinline__ void fc_block(Ring<FAST>& rg, const Cons& c, float (&x)[4][32],
+                                         const float* __restrict__ b0, const int* status) {
   const uint64_t desc0 = make_desc(0);
   float h[32];
 #pragma unroll 1
@@ -317,7 +339,7 @@ __device__ __forceinline__ void fc_block(Ring& rg, const Cons& c, float (&x)[4][
       const uint64_t b_lo = desc0 + ((rg.slot_addr(rg.seq + 1) + c.wg * 8192) >> 4);
       fence_acc<32>(h);
       wgmma_fence();
-      mma3<4>(h, a_hi, b_hi, b_lo, j == 0);
+      mma3<FAST, 4>(h, a_hi, b_hi, b_lo, j == 0);
       rg.issued();
     }
     rg.drain();
@@ -329,6 +351,10 @@ __device__ __forceinline__ void fc_block(Ring& rg, const Cons& c, float (&x)[4][
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const float2 bb = __ldg(reinterpret_cast<const float2*>(bc + 8 * (i >> 2)));
+      if (FAST) {
+        st_shared_u32(acc_addr(ah, 0, i), relu_f16x2(h[i] * c.w_inv + bb.x, h[i + 1] * c.w_inv + bb.y));
+        continue;
+      }
       uint32_t hi, lo;
       split_relu2(h[i] * c.w_inv + bb.x, h[i + 1] * c.w_inv + bb.y, hi, lo);
       const uint32_t a = acc_addr(ah, 0, i);
@@ -340,7 +366,7 @@ __device__ __forceinline__ void fc_block(Ring& rg, const Cons& c, float (&x)[4][
     // ---- X += relu(H_c) W1[:, 128 hc, +128)^T ----
 #pragma unroll 1
     for (int jj = 0; jj < 2; ++jj)
-      wide_steps<4>(rg, c, x, desc0 + ((c.smem_u + SM_AH + jj * A_CHUNK_BYTES) >> 4), false);
+      wide_steps<FAST, 4>(rg, c, x, desc0 + ((c.smem_u + SM_AH + jj * A_CHUNK_BYTES) >> 4), false);
   }
 }
 
@@ -388,8 +414,8 @@ __device__ __forceinline__ void stage_gather(uint32_t smem_u, const float* __res
 // Epilogue of a layer that ends on the residual stream: y = X / s + (gathered projected latent | bias), then
 //   GATHER / BIAS_WB: X = y, relu(y) -> fp16 hi/lo A operand;   COMBINE: view sum (mean after the last view), ditto
 //   OUT: lin_out partial sums of relu(y) into out_part.
-template <int MODE>
-__device__ __forceinline__ void epilogue_x(Ring& rg, const Cons& c, float (&x)[4][32], const float* __restrict__ bias,
+template <bool FAST, int MODE>
+__device__ __forceinline__ void epilogue_x(Ring<FAST>& rg, const Cons& c, float (&x)[4][32], const float* __restrict__ bias,
                                            const float* __restrict__ proj_i, const float* __restrict__ lin_out_w,
                                            int view, int NS, float* __restrict__ scratch, float* out_part) {
   rg.drain();
@@ -459,6 +485,10 @@ __device__ __forceinline__ void epilogue_x(Ring& rg, const Cons& c, float (&x)[4
       } else if (produce) {
         x[q][i] = y0 * c.w_scale;
         x[q][i + 1] = y1 * c.w_scale;
+        if (FAST) {
+          st_shared_u32(acc_addr(xa, q, i), relu_f16x2(y0, y1));
+          continue;
+        }
         uint32_t hi, lo;
         split_relu2(y0, y1, hi, lo);
         const uint32_t a = acc_addr(xa, q, i);
@@ -545,7 +575,8 @@ __device__ __forceinline__ void finish_ray(const Params& p, int ps, int64_t ray,
   }
 }
 
-__global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant__ Params p) {
+template <bool FAST>
+__device__ __forceinline__ void field_tc(const Params& p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = blockIdx.x & 1;        // which 64 points of the 128-point tile
   const int pair = blockIdx.x >> 1;
@@ -580,8 +611,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant_
   __syncthreads();
   if (threadIdx.x == 0) {
     // prefill: steps 0 and 1 (the EMPTY waits of the first use of a slot return at once)
-    feed_step(bar_base, smem_u32(smem + SM_B), 0, p.status);
-    feed_step(bar_base, smem_u32(smem + SM_B), 2, p.status);
+    feed_step<FAST>(bar_base, smem_u32(smem + SM_B), 0, p.status);
+    feed_step<FAST>(bar_base, smem_u32(smem + SM_B), 2, p.status);
   }
   const size_t map_stride = (size_t)p.sc.SB * NS * p.sc.Hl * p.sc.Wl * D;
 
@@ -594,7 +625,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant_
     c.r0 = 16 * (warp & 3) + (lane >> 2);
     c.c0 = 2 * (lane & 3);
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(c.l2_keep));
-    Ring rg;
+    Ring<FAST> rg;
     rg.bar_base = bar_base;
     rg.b_base = smem_u32(smem + SM_B);
     rg.seq = 0;
@@ -692,7 +723,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant_
               const uint32_t lo = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
               const uint32_t byte = swz(grow, ch);
               *reinterpret_cast<uint32_t*>(row_hi - grow * 128 + byte) = hi;
-              *reinterpret_cast<uint32_t*>(row_lo - grow * 128 + byte) = lo;
+              if (!FAST) *reinterpret_cast<uint32_t*>(row_lo - grow * 128 + byte) = lo;   // (FAST: lo is dead)
             }
             fence_proxy_async();
             workers_sync();  // geometry and the lin_in operand visible to both warpgroups
@@ -702,21 +733,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant_
           for (int q = 0; q < 4; ++q)
 #pragma unroll
             for (int i = 0; i < 32; ++i) x[q][i] = 0.f;   // X is dead until here: no registers held across the geometry
-          wide_steps<3>(rg, c, x, a0_desc, true);
-          epilogue_x<MODE_GATHER>(rg, c, x, nullptr, P.proj, nullptr, v, NS, nullptr, nullptr);
+          wide_steps<FAST, 3>(rg, c, x, a0_desc, true);
+          epilogue_x<FAST, MODE_GATHER>(rg, c, x, nullptr, P.proj, nullptr, v, NS, nullptr, nullptr);
           for (int blk = 0; blk < 3; ++blk) {
             fc_block(rg, c, x, P.fc0_b[blk], p.status);
             if (blk < 2)
-              epilogue_x<MODE_GATHER>(rg, c, x, nullptr, P.proj + (size_t)(blk + 1) * map_stride, nullptr, v, NS,
-                                      nullptr, nullptr);
+              epilogue_x<FAST, MODE_GATHER>(rg, c, x, nullptr, P.proj + (size_t)(blk + 1) * map_stride, nullptr, v,
+                                            NS, nullptr, nullptr);
             else
-              epilogue_x<MODE_COMBINE>(rg, c, x, P.fc1_b[2], nullptr, nullptr, v, NS, scratch, nullptr);
+              epilogue_x<FAST, MODE_COMBINE>(rg, c, x, P.fc1_b[2], nullptr, nullptr, v, NS, scratch, nullptr);
           }
         }
         fc_block(rg, c, x, P.fc0_b[3], p.status);
-        epilogue_x<MODE_BIAS_WB>(rg, c, x, P.fc1_b[3], nullptr, nullptr, 0, NS, nullptr, nullptr);
+        epilogue_x<FAST, MODE_BIAS_WB>(rg, c, x, P.fc1_b[3], nullptr, nullptr, 0, NS, nullptr, nullptr);
         fc_block(rg, c, x, P.fc0_b[4], p.status);
-        epilogue_x<MODE_OUT>(rg, c, x, P.fc1_b[4], nullptr, P.lin_out_w, 0, NS, nullptr, out_part);
+        epilogue_x<FAST, MODE_OUT>(rg, c, x, P.fc1_b[4], nullptr, P.lin_out_w, 0, NS, nullptr, out_part);
         if (threadIdx.x < ROWS) {
           const int64_t opt = tile * TILE_POINTS + rank * ROWS + threadIdx.x;
           if (opt < P.total_points) {
@@ -770,6 +801,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant_
     }
   }
 }
+
+// The exact engine (PNR_ENGINE_TC, 3 tensor passes per step) and the single-pass engine (PNR_ENGINE_TC_FAST).
+__global__ void __launch_bounds__(NTHREADS, 1) k_field_tc(const __grid_constant__ Params p) { field_tc<false>(p); }
+__global__ void __launch_bounds__(NTHREADS, 1) k_field_tc_fast(const __grid_constant__ Params p) { field_tc<true>(p); }
 
 // ---------------------------------------------------------------------------------------
 // weight packing: fp32 [512][K] -> fp16 hi/lo 16 KB slots (128 rows x 64 k, 128B-swizzled) in consumption order
@@ -908,25 +943,26 @@ static void fill_pass(tc::Pass& P, const PnrMlp& mlp, const float* proj, float* 
   P.K = K;
 }
 
-static int tc_launch(tc::Params& p, int pairs, cudaStream_t s) {
+static int tc_launch(tc::Params& p, int pairs, bool fast, cudaStream_t s) {
   int rc = tc::get_status_buffer(&p.status);
   if (rc) return rc;
-  static bool attr_set[64] = {false};
+  static bool attr_set[2][64] = {{false}};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (!attr_set[dev]) {
-    PNR_CUDA(cudaFuncSetAttribute(tc::k_field_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
-    attr_set[dev] = true;
+  void (*kernel)(tc::Params) = fast ? tc::k_field_tc_fast : tc::k_field_tc;
+  if (!attr_set[fast][dev]) {
+    PNR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
+    attr_set[fast][dev] = true;
   }
   prof_before(s);
-  tc::k_field_tc<<<dim3(pairs * 2), dim3(tc::NTHREADS), tc::SMEM_BYTES, s>>>(p);
+  kernel<<<dim3(pairs * 2), dim3(tc::NTHREADS), tc::SMEM_BYTES, s>>>(p);
   prof_after(s);
   PNR_LAUNCH_CHECK();
   return PNR_OK;
 }
 
-int tc_field_eval(const PnrScene& sc, const PnrMlp& mlp, const float* proj, const PointSource& src,
-                  int64_t total_points, float* out, void* ws, size_t ws_bytes, cudaStream_t s) {
+static int tc_field_launch(const PnrScene& sc, const PnrMlp& mlp, const float* proj, const PointSource& src,
+                           int64_t total_points, float* out, void* ws, size_t ws_bytes, bool fast, cudaStream_t s) {
   if (!tc_supported(sc, mlp) || !mlp.packed || !proj) {
     set_error("tensor engine: unsupported shape or missing packed weights / projected latent");
     return PNR_ERR_UNSUPPORTED;
@@ -947,7 +983,17 @@ int tc_field_eval(const PnrScene& sc, const PnrMlp& mlp, const float* proj, cons
   fill_pass(p.pass[0], mlp, proj, out, total_points, src.P, src.K > 0 ? src.K : 1);
   p.rn.rays = nullptr;
   p.scratch = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
-  return tc_launch(p, tc_pairs(p.pass[0].n_tiles), s);
+  return tc_launch(p, tc_pairs(p.pass[0].n_tiles), fast, s);
+}
+
+int tc_field_eval(const PnrScene& sc, const PnrMlp& mlp, const float* proj, const PointSource& src,
+                  int64_t total_points, float* out, void* ws, size_t ws_bytes, cudaStream_t s) {
+  return tc_field_launch(sc, mlp, proj, src, total_points, out, ws, ws_bytes, false, s);
+}
+
+int tc_field_eval_fast(const PnrScene& sc, const PnrMlp& mlp, const float* proj, const PointSource& src,
+                       int64_t total_points, float* out, void* ws, size_t ws_bytes, cudaStream_t s) {
+  return tc_field_launch(sc, mlp, proj, src, total_points, out, ws, ws_bytes, true, s);
 }
 
 // ---- fused render: NeRFRenderer.forward (nerf.py:251-303) in ONE launch of the tensor engine ----------------------
@@ -1033,7 +1079,7 @@ int tc_render(const PnrScene& sc, const PnrMlp& mc, const PnrMlp& mf, const floa
   rn.Kfd = Kfd;
   rn.white = cfg.white_bkgd;
   rn.depth_std = cfg.depth_std;
-  return tc_launch(p, pairs, s);
+  return tc_launch(p, pairs, cfg.engine == PNR_ENGINE_TC_FAST, s);
 }
 
 }  // namespace pnr

@@ -343,6 +343,7 @@ int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrSh
   };
   PNR_CHECK_ARG(B >= 0, "B must be >= 0");
   PNR_CHECK_ARG(cfg->n_coarse >= 1 && cfg->n_fine >= 0, "bad sample counts");
+  if (int rc = check_backward_engine(cfg->engine)) return rc;
   DevGuard guard;
   const int n = (int)h->dev.size();
   const int SB = shards[0].scene ? shards[0].scene->SB : 0;

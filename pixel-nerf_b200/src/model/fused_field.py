@@ -68,6 +68,7 @@ class _FusedField(torch.autograd.Function):
 
 
 def fused_field(net, xyz, coarse, viewdirs):
+    pn.check_trainable(net.engine)
     use_fine = (not coarse) and net.mlp_fine is not None
     mlp = net.mlp_fine if use_fine else net.mlp_coarse
     latent = net.encoder.latent.detach() if net.stop_encoder_grad else net.encoder.latent

@@ -93,7 +93,7 @@ class PixelNeRFNet(torch.nn.Module):
         self._image_wh = (0.0, 0.0)
         self._scene_epoch = 0          # bumped by every encode() / set_scene() / set_cameras(): keys per-GPU replicas
         self._fused = _FusedCache()
-        self.engine = os.environ.get("PNR_ENGINE", "auto")  # auto | simt | tc
+        self.engine = os.environ.get("PNR_ENGINE", "auto")  # auto | simt | tc | tc_fast (inference only)
 
     # ------------------------------------------------------------------------------
     # encode(): state producer (models.py:89-144)

@@ -14,8 +14,9 @@ _HERE = os.path.dirname(os.path.realpath(__file__))   # realpath: `src/` may be 
 LIB_PATH = os.environ.get("PNR_LIB", os.path.join(os.path.dirname(_HERE), "lib", "libpnr_sm90.so"))
 
 PNR_MAX_BLOCKS = 8
-ENGINE_AUTO, ENGINE_SIMT, ENGINE_TC = 0, 1, 2
-ENGINES = {"auto": ENGINE_AUTO, "simt": ENGINE_SIMT, "tc": ENGINE_TC}
+ENGINE_AUTO, ENGINE_SIMT, ENGINE_TC, ENGINE_TC_FAST = 0, 1, 2, 4
+# "tc_fast": the single-pass fp16 tensor engine (PNR_ENGINE_TC_FAST), inference only; only ever chosen explicitly
+ENGINES = {"auto": ENGINE_AUTO, "simt": ENGINE_SIMT, "tc": ENGINE_TC, "tc_fast": ENGINE_TC_FAST}
 
 _fp = C.c_void_p  # device pointers travel as void*
 
@@ -200,6 +201,14 @@ def lib():
 def check(rc):
     if rc != 0:
         raise RuntimeError(f"libpnr_sm90 error {rc}: {lib().pnr_last_error().decode()}")
+
+
+def check_trainable(engine):
+    """Raises for an engine whose forward the fused backward cannot reproduce ("tc_fast": its backward would
+    differentiate the exact engine's forward instead), before a grad-mode node runs that forward."""
+    if engine == "tc_fast":
+        raise RuntimeError('engine "tc_fast" is inference only: the single-pass fp16 forward has no matching backward; '
+                           'training needs net.engine = "tc" or "auto" (or run this call under torch.no_grad())')
 
 
 def sync_deterministic():

@@ -139,6 +139,7 @@ class _FusedRender(torch.autograd.Function):
 
 
 def fused_render_train(renderer, model, rays, want_weights, noise_in=None):
+    pn.check_trainable(model.engine)
     fine = bool(renderer.using_fine) and int(renderer.n_fine) > 0
     mlps = [model.mlp_coarse] + ([model.mlp_fine] if (fine and model.mlp_fine is not None) else [])
     params = [p for mlp in mlps for _, p in mlp.named_parameters()]
@@ -388,6 +389,7 @@ def sharded_render_train(sharded, rays, want_weights, noise_in=None):
     dict(u_coarse, u_fine, u_fine_jit, n_depth) of full-ray draws [SB*B][...]; each shard takes its rays' rows (tests
     compare with the single-GPU node on the same draws)."""
     net, renderer = sharded.module.net, sharded.module.renderer
+    pn.check_trainable(net.engine)
     fine = bool(renderer.using_fine) and int(renderer.n_fine) > 0
     mlps = [net.mlp_coarse] + ([net.mlp_fine] if (fine and net.mlp_fine is not None) else [])
     params = [p for mlp in mlps for _, p in mlp.named_parameters()]

@@ -5,11 +5,14 @@ rays, want_weights)`, `bind_parallel(net, gpus, simple_output)`, `sched_step`, m
 
 Inference with a PixelNeRFNet on CUDA runs the whole sample -> field -> composite ->
 resample -> field -> composite chain in one C-ABI call (`pnr_render`, include/pnr.h); the
-random draws are made here with torch, in the reference's order, and handed to the kernels,
-so a seeded run replays the reference's samples.  With autograd enabled (training) on CUDA the
+random draws are made with torch, in the reference's order, and handed to the kernels,
+so a seeded run replays the reference's samples.  render/fused_call.py sets up that call (counts,
+draws, outputs, shards) for every caller.  With autograd enabled (training) on CUDA the
 same fused forward runs inside one autograd node whose backward is `pnr_render_backward_ex`
-(render/fused_train.py), differentiable in rgb, depth and weights like the reference; a foreign `model` callable, CPU tensors in grad mode (host-logic
-tests) or PNR_FUSED_BACKWARD=0 use the composed torch path below.
+(render/fused_train.py), differentiable in rgb, depth and weights like the reference; a foreign
+`model` callable, CPU tensors in grad mode (host-logic tests) or PNR_FUSED_BACKWARD=0 use the
+composed torch path below.  `NeRFRenderer._apply_sched` and `_fused_grad` hold the schedule and
+the choice of that node for both `NeRFRenderer.forward` and `_ShardedRender`.
 
 Multi-GPU (`bind_parallel(net, gpus)`): the reference wraps a `DataParallel(dim=1)`, which
 re-broadcasts the whole module on every call; `_ShardedRender` instead keeps a `_SceneReplica`
@@ -25,6 +28,7 @@ import torch
 
 import pnr_native as pn
 
+from . import fused_call as fc
 from .dotmap_compat import DotMap
 
 
@@ -216,113 +220,34 @@ class _ShardedRender(torch.nn.Module):
             ev[1].record(torch.cuda.current_stream(torch.device("cuda", self.gpus[0])))
             t.setdefault("refresh", []).append(ev)
 
-    def _grad_mode_sharded(self, net, rays):
-        """Training on several GPUs needs the fused node: a PixelNeRFNet, CUDA rays, PNR_FUSED_BACKWARD unset / auto /
-        2 (its other values select single-GPU debugging paths) and no sigma noise (as NeRFRenderer.forward)."""
-        renderer = self.module.renderer
-        return (NeRFRenderer._is_pixelnerf(net) and rays.is_cuda
-                and os.environ.get("PNR_FUSED_BACKWARD", "auto") in ("auto", "2")
-                and not (renderer.training and renderer.noise_std > 0.0))
-
     def forward(self, rays, want_weights=False):
         net, renderer, simple = self.module.net, self.module.renderer, self.module.simple_output
         empty = rays.shape[0] == 0 or rays.shape[1] == 0
         grad = not empty and net._needs_autograd(rays)
-        if empty or (grad and not self._grad_mode_sharded(net, rays)):
+        if empty or (grad and not renderer._fused_grad(net, rays)):
             if grad and not self._warned:
                 warnings.warn(f"bind_parallel(net, {self.gpus}): gradients are required and this model / setting has "
                               f"no sharded backward (it needs a PixelNeRFNet, CUDA rays and PNR_FUSED_BACKWARD unset, "
                               f"auto or 2), so this call runs on cuda:{self.gpus[0]} only")
                 self._warned = True
             return self.module(rays, want_weights=want_weights)
-        if renderer.sched is not None and renderer.last_sched.item() > 0:     # as NeRFRenderer.forward (nerf.py:265-267)
-            renderer.n_coarse = renderer.sched[1][renderer.last_sched.item() - 1]
-            renderer.n_fine = renderer.sched[2][renderer.last_sched.item() - 1]
+        renderer._apply_sched()
         want_weights = want_weights and not simple
         if grad:
             from .fused_train import sharded_render_train
             return _wrapper_output(renderer, sharded_render_train(self, rays, want_weights), simple)
-        Kc, Kf, Kfd = int(renderer.n_coarse), int(renderer.n_fine), int(renderer.n_fine_depth)
-        fine = bool(renderer.using_fine) and Kf > 0
-        if not fine:
-            Kf = Kfd = 0
-        n = len(self.gpus)
+        counts = fc.sample_counts(renderer)
         dev0 = torch.device("cuda", self.gpus[0])
         rays0 = rays.detach().to(dev0).contiguous().float()
         SB, B, _ = rays0.shape
-        cfg = pn.PnrRenderCfg(Kc, Kf, Kfd, float(renderer.depth_std), 1 if renderer.white_bkgd else 0,
-                              pn.ENGINES[net.engine])
-        L = pn.lib()
-
-        def outputs(dev, rays_per_obj):
-            """PnrRenderOut + DotMap of tensors for SB * rays_per_obj rays on `dev` (as NeRFRenderer._forward_fused)."""
-            R = SB * rays_per_obj
-            f32 = dict(dtype=torch.float32, device=dev)
-            o, res = pn.PnrRenderOut(), DotMap()
-            res.coarse = DotMap(rgb=torch.empty(SB, rays_per_obj, 3, **f32), depth=torch.empty(SB, rays_per_obj, **f32))
-            o.rgb_coarse, o.depth_coarse = pn.dptr(res.coarse.rgb), pn.dptr(res.coarse.depth)
-            if want_weights:
-                res.coarse.weights = torch.empty(SB, rays_per_obj, Kc, **f32)
-                o.weights_coarse = pn.dptr(res.coarse.weights)
-            if fine:
-                res.fine = DotMap(rgb=torch.empty(SB, rays_per_obj, 3, **f32), depth=torch.empty(SB, rays_per_obj, **f32))
-                o.rgb_fine, o.depth_fine = pn.dptr(res.fine.rgb), pn.dptr(res.fine.depth)
-                if want_weights:
-                    res.fine.weights = torch.empty(SB, rays_per_obj, Kc + Kf, **f32)
-                    o.weights_fine = pn.dptr(res.fine.weights)
-            return o, res
-
+        cfg = fc.render_cfg(renderer, net.engine)
+        out0, res0 = fc.render_outputs(SB, B, counts, dev0, want_weights, want_z=False)
+        if simple and counts[3]:          # only the best pass is returned: do not ship the other one back
+            out0.rgb_coarse = out0.depth_coarse = None
+        shards, _, keep = fc.setup_shards(self, rays0, counts, cfg, want_weights, want_z=False)
         with torch.cuda.device(dev0):
-            out0, res0 = outputs(dev0, B)
-            if simple:                       # only the best pass is returned: do not ship the other one back
-                if fine:
-                    out0.rgb_coarse = out0.depth_coarse = None
-        shards = (pn.PnrShard * n)()
-        keep = []
-        per = -(-B // n)
-        for i, g in enumerate(self.gpus):
-            Bi = min(B, per * (i + 1)) - min(B, per * i)
-            if Bi <= 0:
-                continue
-            dev = torch.device("cuda", g)
-            model = net
-            if i > 0:
-                model = self._replicas[g]
-                self._refresh(model, fine)
-            with torch.cuda.device(dev):
-                scene, mc, mf, keep2 = model._scene_struct(want_fine=fine)
-                Ri = SB * Bi
-                f32 = dict(dtype=torch.float32, device=dev)
-                noise = pn.PnrNoise()            # draws in the reference's order (nerf.py:111,135,141,158)
-                lin = renderer._lin_steps(Kc, dev)
-                u_c = torch.rand(Ri, Kc, **f32)
-                noise.lin_steps, noise.u_coarse = pn.dptr(lin), pn.dptr(u_c)
-                keep += [lin, u_c, keep2, scene, mc, mf, noise]
-                if fine and Kf - Kfd > 0:
-                    u_f, u_j = torch.rand(Ri, Kf - Kfd, **f32), torch.rand(Ri, Kf - Kfd, **f32)
-                    noise.u_fine, noise.u_fine_jit = pn.dptr(u_f), pn.dptr(u_j)
-                    keep += [u_f, u_j]
-                if fine and Kfd > 0:
-                    n_d = torch.randn(Ri, Kfd, **f32)
-                    noise.n_depth = pn.dptr(n_d)
-                    keep.append(n_d)
-                stage, stage_res = outputs(dev, Bi)
-                ws = pn.workspace(dev, L.pnr_render_workspace_bytes(scene, mc, mf, cfg, Bi))
-                sh = shards[i]
-                import ctypes as C
-                sh.scene, sh.mlp_coarse = C.pointer(scene), C.pointer(mc)
-                sh.mlp_fine = C.pointer(mf) if mf is not None else None
-                sh.noise = C.pointer(noise)
-                sh.workspace, sh.workspace_bytes = ws.data_ptr(), ws.numel()
-                if i > 0 or SB > 1:
-                    stage_rays = torch.empty(SB, Bi, 8, **f32)
-                    sh.rays_stage = pn.dptr(stage_rays)
-                    keep.append(stage_rays)
-                sh.stage = stage
-                sh.stream = pn.stream_ptr(dev)
-                keep += [stage_res, ws]
-        with torch.cuda.device(dev0):
-            pn.check(L.pnr_mgpu_render(self._mgpu(), shards, cfg, pn.dptr(rays0, "rays"), out0, B, pn.stream_ptr(dev0)))
+            pn.check(pn.lib().pnr_mgpu_render(self._mgpu(), shards, cfg, pn.dptr(rays0, "rays"), out0, B,
+                                              pn.stream_ptr(dev0)))
         self._keep = keep        # staging buffers stay referenced until the next call (their streams are still busy)
         return _wrapper_output(renderer, res0, simple)
 
@@ -378,21 +303,28 @@ class NeRFRenderer(torch.nn.Module):
     # ------------------------------------------------------------------------------------
     def forward(self, model, rays, want_weights=False):
         """rays (SB,B,8) -> DotMap(coarse=DotMap(rgb,depth[,weights]), fine=...) (nerf.py:251-303)."""
-        if self.sched is not None and self.last_sched.item() > 0:
-            self.n_coarse = self.sched[1][self.last_sched.item() - 1]
-            self.n_fine = self.sched[2][self.last_sched.item() - 1]
+        self._apply_sched()
         assert rays.dim() == 3
         if self._can_fuse(model, rays):
             return self._forward_fused(model, rays, want_weights)
-        mode = os.environ.get("PNR_FUSED_BACKWARD", "auto")
-        if (mode in ("auto", "2") and rays.is_cuda and self._is_pixelnerf(model)
-                and not (self.training and self.noise_std > 0.0)):
-            # training step on the GPU (train/train.py:199-215): ONE autograd node, pnr_render forward +
-            # pnr_render_backward_ex (render/fused_train.py), gradients through every output.  PNR_FUSED_BACKWARD=1 keeps the renderer in torch ops with a
-            # fused field node (model/fused_field.py); =0 is the composed-torch path the gradient tests compare with.
+        if self._fused_grad(model, rays):
             from .fused_train import fused_render_train
             return fused_render_train(self, model, rays, want_weights)
         return self._forward_torch(model, rays, want_weights)
+
+    def _apply_sched(self):
+        """Sample counts of the schedule step reached so far (nerf.py:265-267)."""
+        if self.sched is not None and self.last_sched.item() > 0:
+            self.n_coarse = self.sched[1][self.last_sched.item() - 1]
+            self.n_fine = self.sched[2][self.last_sched.item() - 1]
+
+    def _fused_grad(self, model, rays):
+        """Whether grad mode runs the fused autograd node (render/fused_train.py; the training step of
+        train/train.py:199-215, gradients through every output): a PixelNeRFNet, CUDA rays, no sigma noise and
+        PNR_FUSED_BACKWARD unset, auto or 2.  =1 keeps the renderer in torch ops with a fused field node
+        (model/fused_field.py); =0 is the composed-torch path the gradient tests compare with."""
+        return (os.environ.get("PNR_FUSED_BACKWARD", "auto") in ("auto", "2") and rays.is_cuda
+                and self._is_pixelnerf(model) and not (self.training and self.noise_std > 0.0))
 
     @staticmethod
     def _is_pixelnerf(model):
@@ -441,63 +373,17 @@ class NeRFRenderer(torch.nn.Module):
         if not rays.is_cuda:
             raise RuntimeError("the fused render path needs CUDA rays (no CPU fallback); got %s" % dev)
         SB, B, _ = rays.shape
-        R = SB * B
-        Kc, Kf, Kfd = int(self.n_coarse), int(self.n_fine), int(self.n_fine_depth)
-        fine = bool(self.using_fine) and Kf > 0
-        if not fine:
-            Kf = Kfd = 0
+        counts = fc.sample_counts(self)
         rays_c = rays.detach().contiguous().float()
-        f32 = dict(dtype=torch.float32, device=dev)
-        # random draws in the reference's order (nerf.py:111,135,141,158)
-        noise = pn.PnrNoise()
-        lin = self._lin_steps(Kc, dev)
-        draw = noise_in is None
-        u_c = torch.rand(R, Kc, **f32) if draw else noise_in["u_coarse"].to(**f32).contiguous()
-        noise.lin_steps, noise.u_coarse = pn.dptr(lin), pn.dptr(u_c)
-        keep = [lin, u_c]
-        if fine and Kf - Kfd > 0:
-            u_f = torch.rand(R, Kf - Kfd, **f32) if draw else noise_in["u_fine"].to(**f32).contiguous()
-            u_j = torch.rand(R, Kf - Kfd, **f32) if draw else noise_in["u_fine_jit"].to(**f32).contiguous()
-            noise.u_fine, noise.u_fine_jit = pn.dptr(u_f), pn.dptr(u_j)
-            keep += [u_f, u_j]
-        if fine and Kfd > 0:
-            n_d = torch.randn(R, Kfd, **f32) if draw else noise_in["n_depth"].to(**f32).contiguous()
-            noise.n_depth = pn.dptr(n_d)
-            keep.append(n_d)
-
-        scene, mc, mf, keep2 = model._scene_struct(want_fine=fine)
+        draws = fc.draw_noise(SB * B, counts, dev, noise_in)
+        noise = fc.bind_noise(self._lin_steps(counts[0], dev), draws)
+        scene, mc, mf, keep = model._scene_struct(want_fine=counts[3])
         if scene.SB != SB:
             raise RuntimeError(f"rays have {SB} objects but encode() saw {scene.SB}")
-        cfg = pn.PnrRenderCfg(Kc, Kf, Kfd, float(self.depth_std), 1 if self.white_bkgd else 0,
-                              pn.ENGINES[model.engine])
-        out = pn.PnrRenderOut()
-        res = DotMap()
-        rgb_c, dep_c = torch.empty(R, 3, **f32), torch.empty(R, **f32)
-        out.rgb_coarse, out.depth_coarse = pn.dptr(rgb_c), pn.dptr(dep_c)
-        res.coarse = DotMap(rgb=rgb_c.view(SB, B, 3), depth=dep_c.view(SB, B))
-        if want_weights:
-            w_c = torch.empty(R, Kc, **f32)
-            out.weights_coarse = pn.dptr(w_c)
-            res.coarse.weights = w_c.view(SB, B, Kc)
-        if want_z:
-            z_c = torch.empty(R, Kc, **f32)
-            out.z_coarse = pn.dptr(z_c)
-            res.coarse.z = z_c.view(SB, B, Kc)
-        if fine:
-            rgb_f, dep_f = torch.empty(R, 3, **f32), torch.empty(R, **f32)
-            out.rgb_fine, out.depth_fine = pn.dptr(rgb_f), pn.dptr(dep_f)
-            res.fine = DotMap(rgb=rgb_f.view(SB, B, 3), depth=dep_f.view(SB, B))
-            if want_weights:
-                w_f = torch.empty(R, Kc + Kf, **f32)
-                out.weights_fine = pn.dptr(w_f)
-                res.fine.weights = w_f.view(SB, B, Kc + Kf)
-            if want_z:
-                z_f = torch.empty(R, Kc + Kf, **f32)
-                out.z_fine = pn.dptr(z_f)
-                res.fine.z = z_f.view(SB, B, Kc + Kf)
+        cfg = fc.render_cfg(self, model.engine)
+        out, res = fc.render_outputs(SB, B, counts, dev, want_weights, want_z)
         L = pn.lib()
-        nbytes = L.pnr_render_workspace_bytes(scene, mc, mf, cfg, B)
-        ws = pn.workspace(dev, nbytes)
+        ws = pn.workspace(dev, L.pnr_render_workspace_bytes(scene, mc, mf, cfg, B))
         with torch.cuda.device(dev):
             pn.check(L.pnr_render(scene, mc, mf, cfg, pn.dptr(rays_c, "rays"), noise, out, B, ws.data_ptr(),
                                   ws.numel(), pn.stream_ptr(dev)))

@@ -22,9 +22,10 @@
 //    and the epilogue gathers 4 taps of P_i and adds them to the residual stream.
 //  * 256 threads = two warpgroups (geometry, wgmma, epilogues, ray finishing), so ptxas may give each thread 255
 //    registers: the 160 accumulator registers plus addressing fit, and each step's 9 or 12 wgmma issue back to back
-//    as one commit group.  There is no weight-stream warp: thread 0 refills the 4-slot ring (cp.async.bulk of
-//    pre-swizzled 16 KB weight tiles in consumption order, mbarrier full/empty) whenever a step's slots are released
-//    (struct Ring).  tests/test_tc_codegen.py guards the register budget.
+//    as one commit group.  There is no weight-stream warp: each warpgroup has its own 4-slot ring of the 8 KB halves
+//    of the pre-swizzled 16 KB weight tiles that it multiplies, which its first thread refills (cp.async.bulk in
+//    consumption order, mbarrier full/empty) whenever the warpgroup releases a step's slots (struct Ring).
+//    tests/test_tc_codegen.py guards the register budget.
 //  * k_field_tc_fast (PNR_ENGINE_TC_FAST) is the same body with FAST = true: one tensor pass per step, D += Ahi*Whi
 //    with fp32 accumulation.  It loads only the W_hi tile of each step (the W_lo slot of the ring stays idle) and never
 //    writes the fp16 lo halves of its A operands.  The projected-latent gather (lin_z stays exact), geometry, the view
@@ -53,6 +54,7 @@ constexpr int NCONSUMER_WARPS = 8;       // two warpgroups
 constexpr int NCONSUMERS = NCONSUMER_WARPS * 32;
 constexpr int NTHREADS = NCONSUMERS;     // thread 0 also issues the weight-slot loads (no dedicated streamer warp)
 constexpr int SLOT_BYTES = 16384;        // 128 weight rows x 64 k x fp16
+constexpr int HALF_SLOT_BYTES = SLOT_BYTES / 2;   // rows [64g, 64g+64) of a slot: the half warpgroup g reads
 constexpr int NSLOTS = 4;
 constexpr int A_CHUNK_BYTES = 16384;     // 64 rows x 64 k x fp16, hi then lo
 constexpr int A_BYTES = 8 * A_CHUNK_BYTES;
@@ -68,13 +70,19 @@ constexpr int SM_AH = SM_A + A_BYTES;                   // 131072
 constexpr int SM_B = SM_AH + AH_BYTES;                  // 163840
 constexpr int SM_GEO = SM_B + NSLOTS * SLOT_BYTES;      // [64][8] words: 4 tap offsets + 4 bilinear weights per row
 constexpr int SM_PART = SM_A;                           // lin_out partials [64][2][4] floats alias A chunk 0 (free at tile end)
-constexpr int SM_BAR = SM_GEO + ROWS * 8 * 4;
+constexpr int SM_BAR = SM_GEO + ROWS * 8 * 4;          // [2][BAR_COUNT]: the mbarriers of each warpgroup's ring
 constexpr int BAR_FULL = 0;                             // [NSLOTS]
 constexpr int BAR_EMPTY = BAR_FULL + NSLOTS;            // [NSLOTS]
 constexpr int BAR_COUNT = BAR_EMPTY + NSLOTS;
-constexpr int SM_NLIST = SM_BAR + BAR_COUNT * 8;        // fused render: number of rays this CTA completed in the current pass
-constexpr int SM_FEED = SM_NLIST + 16;                  // struct Feed: the weight-slot cursor of the producer thread
-constexpr int SMEM_BYTES = SM_FEED + 128;
+constexpr int SM_NLIST = SM_BAR + 2 * BAR_COUNT * 8;    // fused render: number of rays this CTA completed in the current pass
+constexpr int SM_FEED = SM_NLIST + 16;                  // struct Feed [2]: the weight-slot cursor of each warpgroup's ring
+constexpr int FEED_BYTES = 128;
+constexpr int SM_PROF = SM_FEED + 2 * FEED_BYTES;       // phase counters of the profile build: [2][PH_COUNT] u64
+#ifdef PNR_TC_PROFILE
+constexpr int SMEM_BYTES = SM_PROF + 128;
+#else
+constexpr int SMEM_BYTES = SM_PROF;
+#endif
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
 constexpr int FLUSH_SCRATCH_BYTES = A_BYTES / NCONSUMER_WARPS;   // per-warp scratch (cdf + merged samples) in the idle A buffer
 
@@ -125,7 +133,46 @@ using namespace tcptx;
 
 enum { MODE_GATHER = 0, MODE_BIAS_WB = 1, MODE_COMBINE = 2, MODE_OUT = 3 };
 
-__device__ __forceinline__ void workers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// Phase profile (built with -DPNR_TC_PROFILE into lib/libpnr_sm90_prof.so, scripts/tc_phase_profile.py): the first
+// thread of each warpgroup adds the clock64() time it spends in each phase to a shared-memory counter and, at kernel
+// end, to the 8 counters that pnr_tc_counters returns.  The phases are disjoint; the rest of PH_TOTAL is wgmma issue,
+// the epilogue arithmetic and the refill's cursor walk.  The hooks are macros that the production build expands to
+// nothing, so its kernels are the same instructions with or without them (tests/test_tc_profile.py).
+#ifdef PNR_TC_PROFILE
+extern __shared__ __align__(1024) uint8_t smem[];
+enum { PH_FULL, PH_EMPTY, PH_WGMMA_WAIT, PH_SYNC, PH_GATHER, PH_GEOM, PH_FLUSH, PH_TOTAL, PH_COUNT };
+__device__ __forceinline__ void prof_add(int ph, long long t0) {
+  const long long dt = clock64() - t0;
+  if ((threadIdx.x & 127) == 0)
+    reinterpret_cast<unsigned long long*>(smem + SM_PROF)[(threadIdx.x >> 7) * PH_COUNT + ph] += (unsigned long long)dt;
+}
+__device__ __forceinline__ void prof_finish(int* status, long long t_kernel) {
+  prof_add(PH_TOTAL, t_kernel);
+  if ((threadIdx.x & 127) == 0) {
+    const unsigned long long* c = reinterpret_cast<const unsigned long long*>(smem + SM_PROF) + (threadIdx.x >> 7) * PH_COUNT;
+    for (int i = 0; i < PH_COUNT; ++i) atomicAdd(reinterpret_cast<unsigned long long*>(status + 2) + i, c[i]);
+  }
+}
+#define PROF_BEGIN(t) long long t = clock64()
+#define PROF_RESTART(t) t = clock64()
+#define PROF_END(ph, t) prof_add(ph, t)
+// before the kernel's first __syncthreads
+#define PROF_INIT() \
+  if (threadIdx.x < 2 * PH_COUNT) reinterpret_cast<unsigned long long*>(smem + SM_PROF)[threadIdx.x] = 0
+#define PROF_FINISH(status, t) prof_finish(status, t)
+#else
+#define PROF_BEGIN(t)
+#define PROF_RESTART(t)
+#define PROF_END(ph, t)
+#define PROF_INIT()
+#define PROF_FINISH(status, t)
+#endif
+
+__device__ __forceinline__ void workers_sync() {
+  PROF_BEGIN(t0);
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  PROF_END(PH_SYNC, t0);
+}
 
 __device__ __forceinline__ void st_evict_last(float* q, float v, uint64_t pol) {
   asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(q), "f"(v), "l"(pol) : "memory");
@@ -133,6 +180,13 @@ __device__ __forceinline__ void st_evict_last(float* q, float v, uint64_t pol) {
 __device__ __forceinline__ float ld_evict_last(const float* q, uint64_t pol) {
   float v;
   asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(q), "l"(pol) : "memory");
+  return v;
+}
+__device__ __forceinline__ float4 ldg_stream4(const float4* q, uint64_t pol) {
+  float4 v;
+  asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "l"(q), "l"(pol));
   return v;
 }
 __device__ __forceinline__ void st_shared_u32(uint32_t saddr, uint32_t v) {
@@ -160,8 +214,9 @@ __device__ __forceinline__ uint32_t swz(int m, int k) {
 extern __shared__ __align__(1024) uint8_t smem[];
 
 // The weight-slot sequence of one CTA, in consumption order: per pass, per tile of its pair, NS x (lin_in + blocks
-// 0-2: slots [0, 392) of the pass's weight image) then blocks 3-4 (slots [392, 648)).  Thread 0 walks it one slot at a
-// time; the cursor lives in shared memory so that no register is held for it across the MMA loops.
+// 0-2: slots [0, 392) of the pass's weight image) then blocks 3-4 (slots [392, 648)).  Each warpgroup's producer
+// thread walks it one slot at a time with its own cursor; the cursors live in shared memory so that no register is
+// held for them across the MMA loops.
 struct Feed {
   const uint8_t* slots[2];   // first slot of each pass's weight image
   int64_t n_tiles[2];
@@ -175,28 +230,37 @@ struct Feed {
     }
   }
 };
-static_assert(sizeof(Feed) <= SMEM_BYTES - SM_FEED, "Feed does not fit its shared-memory slot");
-__device__ __forceinline__ Feed& feed() { return *reinterpret_cast<Feed*>(smem + SM_FEED); }
+static_assert(sizeof(Feed) <= FEED_BYTES, "Feed does not fit its shared-memory slot");
+static_assert(SM_PROF <= SMEM_BYTES, "the two rings' barriers and cursors fit under the block limit");
+__device__ __forceinline__ Feed& feed(int wg) { return *reinterpret_cast<Feed*>(smem + SM_FEED + wg * FEED_BYTES); }
 
-// Producer (thread 0 only): load the two slots of the step whose first slot has sequence number n, once the slots'
-// previous contents (sequence numbers n - 4, n - 3) are released by all 8 warps.  The single-pass engine loads the
-// W_hi slot only (even sequence numbers: the weight image stores every tile as hi, lo) and steps the cursor over W_lo.
+// Producer of warpgroup wg's ring (thread 128 wg only): load the warpgroup's halves of the two slots of the step whose
+// first slot has sequence number n, once the halves' previous contents (sequence numbers n - 4, n - 3) are released by
+// the warpgroup's 4 warps.  The single-pass engine loads the W_hi slot only (even sequence numbers: the weight image
+// stores every tile as hi, lo) and steps the cursor over W_lo.
 template <bool FAST>
-__device__ __forceinline__ void feed_step(uint32_t bar_base, uint32_t b_base, uint32_t n, int* status) {
-  Feed& f = feed();
+__device__ __forceinline__ void feed_step(uint32_t bar_base, uint32_t b_base, uint32_t n, int wg, int* status) {
+  Feed& f = feed(wg);
 #pragma unroll 1
   for (uint32_t s = n; s < n + 2; ++s) {
     if (f.ps >= f.npass) return;
     const bool load = !FAST || s % 2 == 0;
     const uint32_t sl = s % NSLOTS, ph = (s / NSLOTS) & 1;
-    if (load) mbar_wait(bar_base + (BAR_EMPTY + sl) * 8, ph ^ 1, status, 400 + sl);
+    PROF_BEGIN(t0);
+    if (load) mbar_wait(bar_base + (BAR_EMPTY + sl) * 8, ph ^ 1, status, 410 + 4 * wg + sl);
+    PROF_END(PH_EMPTY, t0);
     const uint32_t full = bar_base + (BAR_FULL + sl) * 8;
     const bool head = f.v < f.NS;   // lin_in + blocks 0-2 of view v, else blocks 3-4
     if (load) {
-      mbar_expect_tx(full, SLOT_BYTES);
-      bulk_g2s(b_base + sl * SLOT_BYTES,
-               f.slots[f.ps] + (size_t)((head ? 0 : SLOTS_LIN_IN + 3 * SLOTS_BLOCK) + f.i) * SLOT_BYTES, SLOT_BYTES,
-               full);
+      // every CTA streams the same 2 x 10 MB of weight images; keep them in L2 ahead of the projected maps that the
+      // gather streams past them (evict_first, stage_gather)
+      uint64_t keep;
+      asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(keep));
+      mbar_expect_tx(full, HALF_SLOT_BYTES);
+      bulk_g2s_hint(b_base + sl * SLOT_BYTES,
+                    f.slots[f.ps] + (size_t)((head ? 0 : SLOTS_LIN_IN + 3 * SLOTS_BLOCK) + f.i) * SLOT_BYTES +
+                        wg * HALF_SLOT_BYTES,
+                    HALF_SLOT_BYTES, full, keep);
     }
     if (++f.i == (head ? SLOTS_LIN_IN + 3 * SLOTS_BLOCK : 2 * SLOTS_BLOCK)) {
       f.i = 0;
@@ -209,21 +273,28 @@ __device__ __forceinline__ void feed_step(uint32_t bar_base, uint32_t b_base, ui
   }
 }
 
-// Weight ring: 4 slots, filled in exactly the order the consumers use them; every step of a consumer warpgroup takes
-// two consecutive slots (W_hi, W_lo of one 128-row x 64-k tile).  A step's slots are released once the wgmma that read
-// them has completed (one step later: wait_group 1, or at the drain that ends an MMA run), and the release refills
-// them with the step two ahead: thread 0 waits until all 8 warps have released them (EMPTY), then issues the
-// cp.async.bulk.  Steps 0 and 1 are loaded at kernel start.
-// This EMPTY wait cannot deadlock: when thread 0 waits in the release of step s, warpgroup 1 still has to release s,
-// which it does in its own `issued` of step s+1 or its drain after step s, with no workers_sync in between (both
-// warpgroups run the same step sequence and every MMA run ends with a drain before the next workers_sync).  To get
-// there it needs only FULL of step s+1, and that load was issued at the release of step s-1, earlier in program order
-// of thread 0.  Warps 1-3 of warpgroup 0 arrive before they reach the next wgmma, so they do not wait on warp 0.
+// Weight rings: one per warpgroup.  Warpgroup g multiplies only rows [64g, 64g+64) of every 128-row weight tile, the
+// contiguous 8 KB at byte 8192 g of each 16 KB slot, so each warpgroup streams its own halves of the 4 slots
+// with its own FULL / EMPTY mbarriers and its own Feed cursor; the two rings share nothing.  The halves are filled in
+// exactly the order the warpgroup uses them; every step takes two consecutive slots (W_hi, W_lo of one 128-row x 64-k
+// tile).  A step's halves are released once the wgmma that read them have completed (one step later: wait_group 1, or
+// at the drain that ends an MMA run), and the release refills them with the step two ahead: the warpgroup's first
+// thread (0 or 128) waits until the warpgroup's 4 warps have released them (EMPTY), then issues the cp.async.bulk.
+// Steps 0 and 1 are loaded at kernel start.  A warpgroup never waits for the other one's refill, so the two may drift
+// apart by up to a step between two workers_sync, which staggers their use of the tensor pipe and of L2.
+// This EMPTY wait cannot deadlock: it depends only on the waiting thread's own warpgroup.  When thread 128g waits in
+// the release of step s, it has released s itself; warps 1-3 of its warpgroup release s in their `issued` of step
+// s+1 or their drain after step s, with no workers_sync in between (every MMA run ends with a drain before the next
+// workers_sync).  To get there they need only FULL of step s+1, whose load thread 128g issued at the release of step
+// s-1, earlier in its own program order, and the wgmma of step s+1, which warp 0 issued before it waited.  The same
+// holds across the pass change: the releases of the coarse pass's last two steps load the fine pass's first two
+// (the cursor runs on into the next pass), and those EMPTY waits are satisfied by the drains that end the coarse
+// pass's last MMA run, before the flush and its workers_sync.
 // FAST (single-pass engine): the same sequence numbers and the same protocol on each step's first (W_hi) slot only;
 // the barriers of the W_lo slots are never used.
 template <bool FAST>
 struct Ring {
-  uint32_t bar_base, b_base;
+  uint32_t bar_base, b_base;   // this warpgroup's barriers; its half of slot 0
   uint32_t seq;      // slot sequence number of the next step
   uint32_t pend;     // first slot of the step still in flight (valid if has_pend)
   bool has_pend;
@@ -231,29 +302,36 @@ struct Ring {
   int* status;
   __device__ __forceinline__ uint32_t slot_addr(uint32_t s) const { return b_base + (s % NSLOTS) * SLOT_BYTES; }
   __device__ __forceinline__ void acquire() {
+    PROF_BEGIN(t0);
     for (uint32_t s = seq; s < seq + (FAST ? 1 : 2); ++s)
-      mbar_wait(bar_base + (BAR_FULL + s % NSLOTS) * 8, (s / NSLOTS) & 1, status, 200 + (int)(s % NSLOTS));
+      mbar_wait(bar_base + (BAR_FULL + s % NSLOTS) * 8, (s / NSLOTS) & 1, status,
+                210 + 4 * (int)(threadIdx.x >> 7) + (int)(s % NSLOTS));
+    PROF_END(PH_FULL, t0);
   }
   __device__ __forceinline__ void release(uint32_t s) {
     __syncwarp();
     if (lane == 0) {
       mbar_arrive(bar_base + (BAR_EMPTY + s % NSLOTS) * 8);
       if (!FAST) mbar_arrive(bar_base + (BAR_EMPTY + (s + 1) % NSLOTS) * 8);
-      if (threadIdx.x == 0) feed_step<FAST>(bar_base, b_base, s + NSLOTS, status);
+      if ((threadIdx.x & 127) == 0) feed_step<FAST>(bar_base, b_base, s + NSLOTS, threadIdx.x >> 7, status);
     }
     __syncwarp();
   }
   // after the step's wgmma are issued: commit them as one group, retire the previous step
   __device__ __forceinline__ void issued() {
     wgmma_commit();
+    PROF_BEGIN(t0);
     wgmma_wait<1>();
+    PROF_END(PH_WGMMA_WAIT, t0);
     if (has_pend) release(pend);
     pend = seq;
     has_pend = true;
     seq += 2;
   }
   __device__ __forceinline__ void drain() {
+    PROF_BEGIN(t0);
     wgmma_wait<0>();
+    PROF_END(PH_WGMMA_WAIT, t0);
     if (has_pend) release(pend);
     has_pend = false;
   }
@@ -313,8 +391,8 @@ __device__ __forceinline__ void wide_steps(Ring<FAST>& rg, const Cons& c, float 
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     rg.acquire();
-    const uint64_t b_hi = desc0 + ((rg.slot_addr(rg.seq) + c.wg * 8192) >> 4);
-    const uint64_t b_lo = desc0 + ((rg.slot_addr(rg.seq + 1) + c.wg * 8192) >> 4);
+    const uint64_t b_hi = desc0 + (rg.slot_addr(rg.seq) >> 4);
+    const uint64_t b_lo = desc0 + (rg.slot_addr(rg.seq + 1) >> 4);
     fence_acc<32>(x[q]);
     wgmma_fence();
     mma3<FAST, KSTEPS>(x[q], a_hi, b_hi, b_lo, zero);
@@ -335,8 +413,8 @@ __device__ __forceinline__ void fc_block(Ring<FAST>& rg, const Cons& c, float (&
     for (int j = 0; j < 8; ++j) {
       rg.acquire();
       const uint64_t a_hi = desc0 + ((c.smem_u + SM_A + j * A_CHUNK_BYTES) >> 4);
-      const uint64_t b_hi = desc0 + ((rg.slot_addr(rg.seq) + c.wg * 8192) >> 4);
-      const uint64_t b_lo = desc0 + ((rg.slot_addr(rg.seq + 1) + c.wg * 8192) >> 4);
+      const uint64_t b_hi = desc0 + (rg.slot_addr(rg.seq) >> 4);
+      const uint64_t b_lo = desc0 + (rg.slot_addr(rg.seq + 1) >> 4);
       fence_acc<32>(h);
       wgmma_fence();
       mma3<FAST, 4>(h, a_hi, b_hi, b_lo, j == 0);
@@ -376,6 +454,8 @@ __device__ __forceinline__ void fc_block(Ring<FAST>& rg, const Cons& c, float (&
 // exactly the two 16-byte units (hi, lo) that the fp16 split of those 8 features overwrites later.
 __device__ __forceinline__ void stage_gather(uint32_t smem_u, const float* __restrict__ proj_i, int warp, int lane) {
   const int sub = lane >> 4, l16 = lane & 15;
+  uint64_t stream;   // the maps (2 x 50 MB at C2) pass through L2 without pushing out the weight images
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(stream));
 #pragma unroll 1
   for (int j = 0; j < 8; ++j) {
     float4 t[4][4];
@@ -396,7 +476,8 @@ __device__ __forceinline__ void stage_gather(uint32_t smem_u, const float* __res
 #pragma unroll
     for (int it = 0; it < 4; ++it)
 #pragma unroll
-      for (int k = 0; k < 4; ++k) t[it][k] = __ldg(reinterpret_cast<const float4*>(proj_i + geo[it][k] + j * 64) + l16);
+      for (int k = 0; k < 4; ++k)
+        t[it][k] = ldg_stream4(reinterpret_cast<const float4*>(proj_i + geo[it][k] + j * 64) + l16, stream);
 #pragma unroll
     for (int it = 0; it < 4; ++it) {
       const int row = warp * 8 + it * 2 + sub;
@@ -424,7 +505,9 @@ __device__ __forceinline__ void epilogue_x(Ring<FAST>& rg, const Cons& c, float 
   workers_sync();   // every warpgroup's wgmma reading the A buffer are complete
   const bool produce = (MODE != MODE_OUT) && !(MODE == MODE_COMBINE && view != NS - 1);
   if (MODE == MODE_GATHER) {
+    PROF_BEGIN(t0);
     stage_gather(c.smem_u, proj_i, c.tid >> 5, c.lane);
+    PROF_END(PH_GATHER, t0);
     workers_sync();
   }
   float o[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
@@ -581,18 +664,22 @@ __device__ __forceinline__ void field_tc(const Params& p) {
   const int rank = blockIdx.x & 1;        // which 64 points of the 128-point tile
   const int pair = blockIdx.x >> 1;
   const int n_pairs = gridDim.x >> 1;
-  const uint32_t bar_base = smem_u32(smem + SM_BAR);
+  const int wg = threadIdx.x >> 7;
+  const uint32_t bar_base = smem_u32(smem + SM_BAR) + wg * BAR_COUNT * 8;   // this warpgroup's ring
+  const uint32_t b_base = smem_u32(smem + SM_B) + wg * HALF_SLOT_BYTES;
   int* n_list = reinterpret_cast<int*>(smem + SM_NLIST);
   const int NS = p.sc.NS;
   const bool render = p.rn.rays != nullptr;
+  PROF_BEGIN(t_kernel);
+  PROF_INIT();
 
-  if (threadIdx.x == 0) {
+  if ((threadIdx.x & 127) == 0) {
     for (int i = 0; i < NSLOTS; ++i) {
       mbar_init(bar_base + (BAR_FULL + i) * 8, 1);
-      mbar_init(bar_base + (BAR_EMPTY + i) * 8, NCONSUMER_WARPS);
+      mbar_init(bar_base + (BAR_EMPTY + i) * 8, NCONSUMER_WARPS / 2);
     }
-    *n_list = 0;
-    Feed& f = feed();
+    if (threadIdx.x == 0) *n_list = 0;
+    Feed& f = feed(wg);
     for (int i = 0; i < 2; ++i) {
       f.slots[i] = i < p.npass ? p.pass[i].packed + HEADER_BYTES : nullptr;
       f.n_tiles[i] = i < p.npass ? p.pass[i].n_tiles : 0;
@@ -609,10 +696,10 @@ __device__ __forceinline__ void field_tc(const Params& p) {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if ((threadIdx.x & 127) == 0) {
     // prefill: steps 0 and 1 (the EMPTY waits of the first use of a slot return at once)
-    feed_step<FAST>(bar_base, smem_u32(smem + SM_B), 0, p.status);
-    feed_step<FAST>(bar_base, smem_u32(smem + SM_B), 2, p.status);
+    feed_step<FAST>(bar_base, b_base, 0, wg, p.status);
+    feed_step<FAST>(bar_base, b_base, 2, wg, p.status);
   }
   const size_t map_stride = (size_t)p.sc.SB * NS * p.sc.Hl * p.sc.Wl * D;
 
@@ -627,7 +714,7 @@ __device__ __forceinline__ void field_tc(const Params& p) {
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(c.l2_keep));
     Ring<FAST> rg;
     rg.bar_base = bar_base;
-    rg.b_base = smem_u32(smem + SM_B);
+    rg.b_base = b_base;
     rg.seq = 0;
     rg.pend = 0;
     rg.has_pend = false;
@@ -645,6 +732,7 @@ __device__ __forceinline__ void field_tc(const Params& p) {
       c.w_scale = reinterpret_cast<const float*>(P.packed)[0];
       c.w_inv = reinterpret_cast<const float*>(P.packed)[1];
       for (int64_t tile = pair; tile < P.n_tiles; tile += n_pairs) {
+        PROF_BEGIN(t_geo);
         const int64_t pt_raw = tile * TILE_POINTS + rank * ROWS + grow;
         const int64_t pt = pt_raw < P.total_points ? pt_raw : P.total_points - 1;
         const int sb = (int)(pt / P.P);
@@ -682,7 +770,9 @@ __device__ __forceinline__ void field_tc(const Params& p) {
               }
               __threadfence();
             }
+            PROF_END(PH_GEOM, t_geo);
             workers_sync();   // every ray of the tile has its merged samples in L2
+            PROF_RESTART(t_geo);
             zz = __ldcg(p.rn.zf + pt);
           }
           for (int i = 0; i < 3; ++i) {
@@ -692,10 +782,12 @@ __device__ __forceinline__ void field_tc(const Params& p) {
         } else {
           load_point(p.src, pt, xp, d);
         }
+        PROF_END(PH_GEOM, t_geo);
         for (int v = 0; v < NS; ++v) {
           // ---- geometry + the 42 input channels -> A chunk 0 (lin_in operand) ----
           workers_sync();   // the previous view / tile is done with the geometry words and A chunk 0
           {
+            PROF_BEGIN(t0);
             PointGeom pg = point_geometry(p.sc, sb, v, xp, d);
             if (gsub == 0) {
               uint32_t* geo = reinterpret_cast<uint32_t*>(smem + SM_GEO) + grow * 8;
@@ -726,6 +818,7 @@ __device__ __forceinline__ void field_tc(const Params& p) {
               if (!FAST) *reinterpret_cast<uint32_t*>(row_lo - grow * 128 + byte) = lo;   // (FAST: lo is dead)
             }
             fence_proxy_async();
+            PROF_END(PH_GEOM, t0);
             workers_sync();  // geometry and the lin_in operand visible to both warpgroups
           }
           // ---- lin_in (overwrites X), then blocks 0..2 ----
@@ -792,14 +885,17 @@ __device__ __forceinline__ void field_tc(const Params& p) {
         const int n_done = *reinterpret_cast<volatile int*>(n_list);
         __threadfence();   // acquire side of the completion counters
         float* fs = reinterpret_cast<float*>(smem + SM_A + warp * FLUSH_SCRATCH_BYTES);
+        PROF_BEGIN(t0);
         for (int i = warp; i < n_done; i += NCONSUMER_WARPS)
           finish_ray(p, ps, p.rn.lists[(size_t)blockIdx.x * p.rn.cap + i], fs, lane);
+        PROF_END(PH_FLUSH, t0);
         workers_sync();
         if (threadIdx.x == 0) *n_list = 0;
         // (the next pass's first write to n_list happens after several workers_sync of its first tile)
       }
     }
   }
+  PROF_FINISH(p.status, t_kernel);
 }
 
 // The exact engine (PNR_ENGINE_TC, 3 tensor passes per step) and the single-pass engine (PNR_ENGINE_TC_FAST).
@@ -1183,8 +1279,9 @@ int pnr_tc_status(int* out) {
 }
 
 
-// Debug: 8 cycle counters accumulated over all launches since the last call; clears them.  The wgmma kernel
-// records none, so they read 0.
+// Debug: 8 cycle counters accumulated over all launches since the last call; clears them.  Only the profile build
+// of the tensor engine (-DPNR_TC_PROFILE, lib/libpnr_sm90_prof.so) records them: its per-phase clocks, PH_FULL ..
+// PH_TOTAL, summed over the first thread of each warpgroup of every CTA.  Otherwise they read 0.
 int pnr_tc_counters(unsigned long long* out8) {
   int* buf = nullptr;
   int rc = tc::get_status_buffer(&buf);

@@ -246,6 +246,19 @@ int pnr_field_backward_cam(const PnrScene* scene, const PnrMlp* mlp, const float
                            const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz,
                            float* d_viewdirs, const PnrCameraGrad* cam, int64_t P, void* workspace,
                            size_t workspace_bytes, void* stream);
+/* pnr_field_backward_cam for a partly frozen network: computes only the gradients that are wanted, each bit-equal to
+ * what pnr_field_backward_cam gives for it.  NULL means frozen:
+ *   grad       : may be NULL (the whole MLP frozen), and so may any of its weight / bias members.  A NULL weight skips
+ *                its weight-gradient GEMM and the two transposes that feed it; a NULL bias skips its row sum.
+ *   d_latent_nhwc, d_xyz, d_viewdirs, cam : as in pnr_field_backward_cam.
+ * The input-gradient chain stops below the lowest layer with a wanted tensor unless d_latent_nhwc, d_xyz, d_viewdirs
+ * or cam is wanted, and the transposed weight copies of layers it does not reach are not made.  dlat = dh Wz runs only
+ * for d_latent_nhwc, d_xyz or cam; the lin_in input GEMM and the geometry backward only for an input gradient.  With
+ * nothing wanted the call returns before the forward recompute.  Same workspace as pnr_field_backward. */
+int pnr_field_backward_sel(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
+                           const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz,
+                           float* d_viewdirs, const PnrCameraGrad* cam, int64_t P, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* Backward of the compositing tail (pnr_composite; oracle/pnr_aux_backward.py::composite_backward): upstream gradients
  * d_rgb [R][3], d_depth [R], d_weights [R][K] (each may be NULL = zero) ->
@@ -286,6 +299,17 @@ int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, cons
  * gradient is computed as well.  Not differentiated: image_shape and latent_scaling (buffers, as in the reference).
  * Same workspace as pnr_render_backward_ex. */
 int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                            const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise,
+                            const PnrRenderOut* fwd, const PnrRenderGrad* up, const PnrMlp* grad_coarse,
+                            const PnrMlp* grad_fine, float* d_latent_nhwc, float* d_rays, const PnrCameraGrad* cam,
+                            int64_t B, void* workspace, size_t workspace_bytes, void* stream);
+/* pnr_render_backward_cam for a partly frozen network (pnr_field_backward_sel's NULL rules): grad_coarse / grad_fine
+ * may be NULL (that MLP frozen), and so may any of their members; wanted gradients are bit-equal to
+ * pnr_render_backward_cam's.  A pass runs (field recompute, compositing backward, field backward) only when it has an
+ * upstream gradient and its MLP has a wanted tensor or d_latent_nhwc, d_rays or cam is wanted.  The fine pass also runs
+ * when depth-centred samples carry d(depth_coarse) to a coarse pass that runs; it then only computes the positions'
+ * gradient for that.  Same workspace as pnr_render_backward_ex. */
+int pnr_render_backward_sel(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
                             const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise,
                             const PnrRenderOut* fwd, const PnrRenderGrad* up, const PnrMlp* grad_coarse,
                             const PnrMlp* grad_fine, float* d_latent_nhwc, float* d_rays, const PnrCameraGrad* cam,
@@ -403,6 +427,13 @@ int pnr_mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardG
  * Camera gradients of every shard are summed onto cam0 by the same reduction as the weights, in shard order.  With
  * d_rays0 and cam0 NULL this is pnr_mgpu_render_backward. */
 int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
+                                 const PnrShardCam* shard_cams, const PnrRenderCfg* cfg, const PnrRenderGrad* up0,
+                                 const PnrMlp* grad_coarse0, const PnrMlp* grad_fine0, float* d_latent0_nhwc,
+                                 float* d_rays0, const PnrCameraGrad* cam0, int64_t B, void* stream0);
+/* pnr_mgpu_render_backward_cam over pnr_render_backward_sel on every shard: grad_coarse0 / grad_fine0 and their members
+ * may be NULL (frozen), and each shard's structs must be NULL in the same places.  The arenas then hold only the wanted
+ * tensors, so the reduction adds fewer floats; an arena_count of 0 (nothing but ray gradients wanted) skips it. */
+int pnr_mgpu_render_backward_sel(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
                                  const PnrShardCam* shard_cams, const PnrRenderCfg* cfg, const PnrRenderGrad* up0,
                                  const PnrMlp* grad_coarse0, const PnrMlp* grad_fine0, float* d_latent0_nhwc,
                                  float* d_rays0, const PnrCameraGrad* cam0, int64_t B, void* stream0);

@@ -80,6 +80,38 @@ static int check_mlp(const PnrMlp* m) {
   return PNR_OK;
 }
 
+// A gradient PnrMlp of the _sel entry points: NULL (the whole MLP frozen) or any of its tensors NULL, with mlp's shape.
+static int check_grad_sel(const PnrMlp* g, const PnrMlp* mlp) {
+  if (!g) return PNR_OK;
+  PNR_CHECK_ARG(g->d_hidden == mlp->d_hidden && g->n_blocks == mlp->n_blocks && g->d_in == mlp->d_in &&
+                    g->d_latent == mlp->d_latent && g->combine_layer == mlp->combine_layer,
+                "grad must have the shape of mlp");
+  return PNR_OK;
+}
+
+// grad, or for NULL a PnrMlp of mlp's shape with every gradient NULL (frozen)
+static PnrMlp grad_or_frozen(const PnrMlp* g, const PnrMlp& mlp) {
+  if (g) return *g;
+  PnrMlp f{};
+  f.d_in = mlp.d_in;
+  f.d_latent = mlp.d_latent;
+  f.d_hidden = mlp.d_hidden;
+  f.d_out = mlp.d_out;
+  f.n_blocks = mlp.n_blocks;
+  f.combine_layer = mlp.combine_layer;
+  return f;
+}
+
+// any tensor of g (a gradient PnrMlp of mlp's shape) is wanted
+static bool any_wanted(const PnrMlp& g) {
+  bool any = g.lin_in_w || g.lin_in_b || g.lin_out_w || g.lin_out_b;
+  for (int i = 0; i < g.n_blocks && i < PNR_MAX_BLOCKS; ++i) {
+    any = any || g.fc0_w[i] || g.fc0_b[i] || g.fc1_w[i] || g.fc1_b[i];
+    if (i < g.combine_layer) any = any || g.lin_z_w[i] || g.lin_z_b[i];
+  }
+  return any;
+}
+
 // engine actually used for (scene, mlp): AUTO prefers the tensor engine when it applies (never the single-pass one).
 static int resolve_engine(const PnrScene& sc, const PnrMlp& mlp, const float* proj, int engine) {
   bool tc_ok = tc_supported(sc, mlp) && mlp.packed != nullptr && proj != nullptr;
@@ -285,17 +317,23 @@ int pnr_field_backward(const PnrScene* scene, const PnrMlp* mlp, const float* xy
                                 workspace, workspace_bytes, stream);
 }
 
-int pnr_field_backward_cam(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
-                           const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz,
-                           float* d_viewdirs, const PnrCameraGrad* cam, int64_t P, void* workspace,
-                           size_t workspace_bytes, void* stream) {
+// pnr_field_backward_cam (sel = false: every gradient of grad is required) and pnr_field_backward_sel (sel = true: NULL
+// grad or NULL members are frozen)
+static int field_backward_entry(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
+                                const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz,
+                                float* d_viewdirs, const PnrCameraGrad* cam, int64_t P, void* workspace,
+                                size_t workspace_bytes, void* stream, bool sel) {
   int rc;
   if ((rc = check_scene(scene))) return rc;
   if ((rc = check_mlp(mlp))) return rc;
-  if ((rc = check_mlp(grad))) return rc;
-  PNR_CHECK_ARG(grad->d_hidden == mlp->d_hidden && grad->n_blocks == mlp->n_blocks && grad->d_in == mlp->d_in &&
-                    grad->d_latent == mlp->d_latent && grad->combine_layer == mlp->combine_layer,
-                "grad must have the shape of mlp");
+  if (sel) {
+    if ((rc = check_grad_sel(grad, mlp))) return rc;
+  } else {
+    if ((rc = check_mlp(grad))) return rc;
+    PNR_CHECK_ARG(grad->d_hidden == mlp->d_hidden && grad->n_blocks == mlp->n_blocks && grad->d_in == mlp->d_in &&
+                      grad->d_latent == mlp->d_latent && grad->combine_layer == mlp->combine_layer,
+                  "grad must have the shape of mlp");
+  }
   PNR_CHECK_ARG(P >= 0, "P must be >= 0");
   if (P == 0) return PNR_OK;
   PNR_CHECK_ARG(xyz && viewdirs && d_out && workspace, "NULL pointer");
@@ -305,8 +343,24 @@ int pnr_field_backward_cam(const PnrScene* scene, const PnrMlp* mlp, const float
   src.dirs = viewdirs;
   src.P = P;
   src.K = 1;
-  return field_backward(*scene, *mlp, src, P * scene->SB, d_out, *grad, d_latent_nhwc, d_xyz, d_viewdirs, cam,
-                        workspace, workspace_bytes, (cudaStream_t)stream);
+  return field_backward(*scene, *mlp, src, P * scene->SB, d_out, grad_or_frozen(grad, *mlp), d_latent_nhwc, d_xyz,
+                        d_viewdirs, cam, workspace, workspace_bytes, (cudaStream_t)stream, sel);
+}
+
+int pnr_field_backward_cam(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
+                           const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz,
+                           float* d_viewdirs, const PnrCameraGrad* cam, int64_t P, void* workspace,
+                           size_t workspace_bytes, void* stream) {
+  return field_backward_entry(scene, mlp, xyz, viewdirs, d_out, grad, d_latent_nhwc, d_xyz, d_viewdirs, cam, P,
+                              workspace, workspace_bytes, stream, false);
+}
+
+int pnr_field_backward_sel(const PnrScene* scene, const PnrMlp* mlp, const float* xyz, const float* viewdirs,
+                           const float* d_out, const PnrMlp* grad, float* d_latent_nhwc, float* d_xyz,
+                           float* d_viewdirs, const PnrCameraGrad* cam, int64_t P, void* workspace,
+                           size_t workspace_bytes, void* stream) {
+  return field_backward_entry(scene, mlp, xyz, viewdirs, d_out, grad, d_latent_nhwc, d_xyz, d_viewdirs, cam, P,
+                              workspace, workspace_bytes, stream, true);
 }
 
 static size_t render_bwd_field_ws(const PnrScene& sc, const PnrMlp& m, int64_t pts) {
@@ -335,15 +389,16 @@ size_t pnr_render_backward_workspace_bytes(const PnrScene* scene, const PnrMlp* 
 }
 
 // argument checks shared by pnr_render_backward and pnr_render_backward_ex, in the order the former always made them
+// (sel: the gradient structs follow pnr_render_backward_sel's rules instead)
 static int check_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
                                  const PnrRenderCfg* cfg, const PnrNoise* noise, const PnrRenderOut* fwd,
-                                 const PnrMlp* grad_coarse, const PnrMlp* grad_fine, int64_t B) {
+                                 const PnrMlp* grad_coarse, const PnrMlp* grad_fine, int64_t B, bool sel = false) {
   int rc;
   if ((rc = check_scene(scene))) return rc;
   if ((rc = check_mlp(mlp_coarse))) return rc;
-  if ((rc = check_mlp(grad_coarse))) return rc;
+  if (sel ? (rc = check_grad_sel(grad_coarse, mlp_coarse)) : (rc = check_mlp(grad_coarse))) return rc;
   if (mlp_fine && (rc = check_mlp(mlp_fine))) return rc;
-  if (mlp_fine && (rc = check_mlp(grad_fine))) return rc;
+  if (mlp_fine && (sel ? (rc = check_grad_sel(grad_fine, mlp_fine)) : (rc = check_mlp(grad_fine)))) return rc;
   PNR_CHECK_ARG(cfg && noise && fwd, "cfg / noise / fwd is NULL");
   PNR_CHECK_ARG(cfg->n_coarse >= 1 && cfg->n_fine >= 0 && cfg->n_fine_depth >= 0 &&
                     cfg->n_fine_depth <= cfg->n_fine,
@@ -360,13 +415,16 @@ int pnr_render_backward_ex(const PnrScene* scene, const PnrMlp* mlp_coarse, cons
                                  d_latent_nhwc, nullptr, nullptr, B, workspace, workspace_bytes, stream);
 }
 
-int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
-                            const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise, const PnrRenderOut* fwd,
-                            const PnrRenderGrad* up, const PnrMlp* grad_coarse, const PnrMlp* grad_fine,
-                            float* d_latent_nhwc, float* d_rays, const PnrCameraGrad* cam, int64_t B, void* workspace,
-                            size_t workspace_bytes, void* stream) {
+// pnr_render_backward_cam (sel = false) and pnr_render_backward_sel (sel = true: NULL gradient structs / members are
+// frozen)
+static int render_backward_entry(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                                 const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise,
+                                 const PnrRenderOut* fwd, const PnrRenderGrad* up, const PnrMlp* grad_coarse,
+                                 const PnrMlp* grad_fine, float* d_latent_nhwc, float* d_rays, const PnrCameraGrad* cam,
+                                 int64_t B, void* workspace, size_t workspace_bytes, void* stream, bool sel) {
   int rc;
-  if ((rc = check_render_backward(scene, mlp_coarse, mlp_fine, cfg, noise, fwd, grad_coarse, grad_fine, B))) return rc;
+  if ((rc = check_render_backward(scene, mlp_coarse, mlp_fine, cfg, noise, fwd, grad_coarse, grad_fine, B, sel)))
+    return rc;
   const int64_t R = B * scene->SB;
   if (R == 0) return PNR_OK;
   const int Kc = cfg->n_coarse, Kf = cfg->n_fine, Kfd = cfg->n_fine_depth, K = Kc + Kf;
@@ -375,6 +433,13 @@ int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, con
   const bool fine_grad = Kf > 0 && (g.d_rgb_fine || g.d_depth_fine || g.d_weights_fine);
   const bool depth_path = fine_grad && Kfd > 0;
   const bool coarse_grad = g.d_rgb_coarse || g.d_depth_coarse || g.d_weights_coarse || depth_path;
+  // ... and so is a pass that has nothing wanted to reach: no trainable tensor in its MLP and no input gradient.  The
+  // fine pass also runs for the coarse pass's sake when depth-centred samples carry d(depth_coarse) over to it.
+  const PnrMlp gc = grad_or_frozen(grad_coarse, *mlp_coarse);
+  const PnrMlp gf = mlp_fine ? grad_or_frozen(grad_fine, *mlp_fine) : gc;
+  const bool want_input = d_latent_nhwc || d_rays || (cam && (cam->d_poses || cam->d_focal || cam->d_c));
+  const bool coarse_run = coarse_grad && (want_input || any_wanted(gc));
+  const bool fine_run = fine_grad && (want_input || any_wanted(gf) || (depth_path && coarse_run));
   PNR_CHECK_ARG(rays && workspace && fwd->z_coarse, "NULL pointer (rays, workspace, z_coarse)");
   if (fine_grad) PNR_CHECK_ARG(fwd->z_fine, "fine-pass gradients need the forward's z_fine");
   if (depth_path) PNR_CHECK_ARG(fwd->depth_coarse && noise->n_depth, "depth samples need depth_coarse and n_depth");
@@ -403,9 +468,8 @@ int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, con
   PointSource src{};
   src.mode = 1;
   src.rays = rays;
-  if (fine_grad) {   // fine pass first: it feeds d(depth_coarse) into the coarse pass (nerf.py:289-291)
+  if (fine_run) {   // fine pass first: it feeds d(depth_coarse) into the coarse pass (nerf.py:289-291)
     const PnrMlp* m = mlp_fine ? mlp_fine : mlp_coarse;
-    const PnrMlp* gm = mlp_fine ? grad_fine : grad_coarse;
     src.z = fwd->z_fine;
     src.K = K;
     src.P = B * K;
@@ -414,8 +478,8 @@ int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, con
     if ((rc = launch_composite_bwd(rays, fwd->z_fine, field, g.d_rgb_fine, g.d_depth_fine, g.d_weights_fine,
                                    cfg->white_bkgd, d_field, d_z, dfar, R, K, s)))
       return rc;
-    if ((rc = field_backward(*scene, *m, src, R * K, d_field, *gm, d_latent_nhwc,
-                             (depth_path || want_rays) ? d_xyz : nullptr, vd, cam, rest, rest_bytes, s)))
+    if ((rc = field_backward(*scene, *m, src, R * K, d_field, gf, d_latent_nhwc,
+                             (depth_path || want_rays) ? d_xyz : nullptr, vd, cam, rest, rest_bytes, s, sel)))
       return rc;
     if (depth_path) {
       if ((rc = launch_depth_grad(rays, fwd->z_fine, fwd->depth_coarse, noise->n_depth, cfg->depth_std, d_z, d_xyz,
@@ -427,8 +491,8 @@ int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, con
                                            noise->n_depth, cfg->depth_std, Kfd, false, d_rays, R, K, s)))
       return rc;
   }
-  if (!coarse_grad) {
-    if (want_rays && !fine_grad) PNR_CUDA(cudaMemsetAsync(d_rays, 0, (size_t)R * 8 * sizeof(float), s));
+  if (!coarse_run) {
+    if (want_rays && !fine_run) PNR_CUDA(cudaMemsetAsync(d_rays, 0, (size_t)R * 8 * sizeof(float), s));
     return PNR_OK;
   }
   src.z = fwd->z_coarse;
@@ -439,12 +503,30 @@ int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, con
   if ((rc = launch_composite_bwd(rays, fwd->z_coarse, field, g.d_rgb_coarse, d_depth_coarse, g.d_weights_coarse,
                                  cfg->white_bkgd, d_field, d_z, dfar, R, Kc, s)))
     return rc;
-  if ((rc = field_backward(*scene, *mlp_coarse, src, R * Kc, d_field, *grad_coarse, d_latent_nhwc,
-                           want_rays ? d_xyz : nullptr, vd, cam, rest, rest_bytes, s)))
+  if ((rc = field_backward(*scene, *mlp_coarse, src, R * Kc, d_field, gc, d_latent_nhwc,
+                           want_rays ? d_xyz : nullptr, vd, cam, rest, rest_bytes, s, sel)))
     return rc;
   if (!want_rays) return PNR_OK;
-  return launch_ray_grad(rays, fwd->z_coarse, d_z, d_xyz, d_vd, d_far, false, nullptr, nullptr, 0.f, 0, fine_grad,
+  return launch_ray_grad(rays, fwd->z_coarse, d_z, d_xyz, d_vd, d_far, false, nullptr, nullptr, 0.f, 0, fine_run,
                          d_rays, R, Kc, s);
+}
+
+int pnr_render_backward_cam(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                            const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise, const PnrRenderOut* fwd,
+                            const PnrRenderGrad* up, const PnrMlp* grad_coarse, const PnrMlp* grad_fine,
+                            float* d_latent_nhwc, float* d_rays, const PnrCameraGrad* cam, int64_t B, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  return render_backward_entry(scene, mlp_coarse, mlp_fine, cfg, rays, noise, fwd, up, grad_coarse, grad_fine,
+                               d_latent_nhwc, d_rays, cam, B, workspace, workspace_bytes, stream, false);
+}
+
+int pnr_render_backward_sel(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,
+                            const PnrRenderCfg* cfg, const float* rays, const PnrNoise* noise, const PnrRenderOut* fwd,
+                            const PnrRenderGrad* up, const PnrMlp* grad_coarse, const PnrMlp* grad_fine,
+                            float* d_latent_nhwc, float* d_rays, const PnrCameraGrad* cam, int64_t B, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  return render_backward_entry(scene, mlp_coarse, mlp_fine, cfg, rays, noise, fwd, up, grad_coarse, grad_fine,
+                               d_latent_nhwc, d_rays, cam, B, workspace, workspace_bytes, stream, true);
 }
 
 int pnr_render_backward(const PnrScene* scene, const PnrMlp* mlp_coarse, const PnrMlp* mlp_fine,

@@ -140,7 +140,7 @@ int check_backward_engine(int engine);
 size_t field_backward_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int64_t total_points);
 int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src, int64_t total_points,
                    const float* d_out, const PnrMlp& grad, float* d_latent, float* d_xyz, float* d_dirs,
-                   const PnrCameraGrad* cam, void* ws, size_t ws_bytes, cudaStream_t s);
+                   const PnrCameraGrad* cam, void* ws, size_t ws_bytes, cudaStream_t s, bool sel = false);
 
 // ---- tensor engine (pnr_field_tc.cu) ---------------------------------------------------
 bool tc_supported(const PnrScene& sc, const PnrMlp& mlp);

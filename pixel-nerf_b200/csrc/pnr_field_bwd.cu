@@ -236,8 +236,8 @@ __global__ void k_geom_bwd(PnrScene sc, PointSource src, int64_t g0, int64_t n_p
     const float w_nw = wx0 * wy0, w_ne = vx1 ? wx1 * wy0 : 0.f, w_sw = vy1 ? wx0 * wy1 : 0.f,
                 w_se = (vx1 && vy1) ? wx1 * wy1 : 0.f;
     float dnw = 0.f, dne = 0.f, dsw = 0.f, dse = 0.f;
-    const float* dl = d_lat + row * C;
-    for (int c = lane; c < C; c += 32) {
+    const float* dl = d_lat ? d_lat + row * C : nullptr;   // NULL: only d_dirs is wanted, which does not read it
+    for (int c = lane; dl && c < C; c += 32) {
       const float gdl = dl[c];
       dnw = fmaf(gdl, sc.latent_nhwc[o_nw + c], dnw);
       dne = fmaf(gdl, sc.latent_nhwc[o_ne + c], dne);
@@ -439,7 +439,7 @@ size_t field_backward_workspace_bytes(const PnrScene& sc, const PnrMlp& mlp, int
 
 int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src, int64_t total_points,
                    const float* d_out, const PnrMlp& grad, float* d_latent, float* d_xyz, float* d_dirs,
-                   const PnrCameraGrad* cam, void* ws, size_t ws_bytes, cudaStream_t s) {
+                   const PnrCameraGrad* cam, void* ws, size_t ws_bytes, cudaStream_t s, bool sel) {
   using namespace bwd;
   PNR_CHECK_ARG(mlp.d_in == 42 && mlp.d_out == 4, "backward expects d_in == 42, d_out == 4");
   PNR_CHECK_ARG(mlp.d_hidden % 16 == 0 && mlp.d_latent % 16 == 0, "d_hidden and d_latent must be multiples of 16");
@@ -467,16 +467,33 @@ int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src
   SplitKScope splitk(b.splitk, b.splitk_bytes);
   const bool want_cam = cam && (cam->d_poses || cam->d_focal || cam->d_c);
   const int V = sc.SB * NS;
+
+  // The plan of a selective call (sel: the _sel entry points): which of the backward's steps its wanted gradients need
+  // (a NULL member of grad is frozen).  The input-gradient chain runs top down through the stages fc_1, fc_0, lin_z of
+  // each block, then lin_in; stage(blk, j) numbers them in that order.  It has to deliver dY to the lowest stage with a
+  // wanted tensor, and all the way down when an input gradient is wanted.  Other calls run every step.
+  auto stage = [&](int blk, int j) { return (nb - 1 - blk) * 3 + j; };
+  const int lin_in_stage = nb * 3;
+  const bool want_dlat = !sel || d_latent || d_xyz || want_cam;     // k_geom_bwd reads dlat for the scatter and d uv
+  const bool want_geom = want_dlat || d_dirs;
+  const bool want_lin_out = grad.lin_out_w || grad.lin_out_b;
+  int reach = want_geom || grad.lin_in_w || grad.lin_in_b ? lin_in_stage : -1;
+  for (int blk = 0; blk < nb; ++blk) {
+    if (grad.fc1_w[blk] || grad.fc1_b[blk]) reach = reach > stage(blk, 0) ? reach : stage(blk, 0);
+    if (grad.fc0_w[blk] || grad.fc0_b[blk]) reach = reach > stage(blk, 1) ? reach : stage(blk, 1);
+    if (blk < comb && (grad.lin_z_w[blk] || grad.lin_z_b[blk])) reach = reach > stage(blk, 2) ? reach : stage(blk, 2);
+  }
+  if (!want_lin_out && reach < 0) return PNR_OK;             // nothing wanted: no recompute either
   if (want_cam) PNR_CUDA(cudaMemsetAsync(b.cam_acc, 0, (size_t)V * 16 * sizeof(float), s));
 
-  // transposed weights, once per call: W [out][in] -> W^T [in][out]
+  // transposed weights, once per call: W [out][in] -> W^T [in][out]; only those of the dX steps the chain runs
   k_pad_rows<<<(d * 48 + 255) / 256, 256, 0, s>>>(mlp.lin_in_w, b.w_in, d, mlp.d_in, 48);
   PNR_LAUNCH_CHECK();
-  BW(transpose_pad<false>(b.w_in, 48, d, 48, b.w_inT, d, s));
+  if (want_geom) BW(transpose_pad<false>(b.w_in, 48, d, 48, b.w_inT, d, s));
   for (int i = 0; i < nb; ++i) {
-    BW(transpose_pad<false>(mlp.fc0_w[i], d, d, d, b.w0T[i], d, s));
-    BW(transpose_pad<false>(mlp.fc1_w[i], d, d, d, b.w1T[i], d, s));
-    if (i < comb) BW(transpose_pad<false>(mlp.lin_z_w[i], L, d, L, b.wzT[i], d, s));
+    if (reach >= stage(i, 2)) BW(transpose_pad<false>(mlp.fc0_w[i], d, d, d, b.w0T[i], d, s));
+    if (reach >= stage(i, 1)) BW(transpose_pad<false>(mlp.fc1_w[i], d, d, d, b.w1T[i], d, s));
+    if (i < comb && want_dlat) BW(transpose_pad<false>(mlp.lin_z_w[i], L, d, L, b.wzT[i], d, s));
   }
 
   for (int64_t g0 = 0; g0 < total_points; g0 += cp) {
@@ -513,24 +530,29 @@ int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src
     k_lin_out_bwd<<<(unsigned)(((int64_t)rows_last * 32 + 255) / 256), 256, 0, s>>>(
         b.hlast, mlp.lin_out_w, mlp.lin_out_b, d_out + g0 * 4, b.do4, b.dh, rows_last, d);
     PNR_LAUNCH_CHECK();
-    BW(transpose_pad<false>(b.do4, 4, rows_last, 4, b.tA, rlp, s));
-    BW(transpose_pad<true>(b.hlast, d, rows_last, d, b.tB, rlp, s));
-    BW(gemm(b.tA, rlp, b.tB, nullptr, const_cast<float*>(grad.lin_out_w), d, 4, d, rlp, false, true, s));
-    BW(rowsum_acc(b.tA, rlp, 4, const_cast<float*>(grad.lin_out_b), s));
-    PNR_CUDA(cudaMemsetAsync(b.dlat, 0, (size_t)R * L * sizeof(float), s));
+    if (want_lin_out) BW(transpose_pad<false>(b.do4, 4, rows_last, 4, b.tA, rlp, s));
+    if (grad.lin_out_w) {
+      BW(transpose_pad<true>(b.hlast, d, rows_last, d, b.tB, rlp, s));
+      BW(gemm(b.tA, rlp, b.tB, nullptr, const_cast<float*>(grad.lin_out_w), d, 4, d, rlp, false, true, s));
+    }
+    if (grad.lin_out_b) BW(rowsum_acc(b.tA, rlp, 4, const_cast<float*>(grad.lin_out_b), s));
+    if (want_dlat) PNR_CUDA(cudaMemsetAsync(b.dlat, 0, (size_t)R * L * sizeof(float), s));
     bool lat_transposed = false;
     float* dh = b.dh;
     float* dh_other = b.dhv;
-    for (int blk = nb - 1; blk >= 0; --blk) {
+    for (int blk = nb - 1; blk >= 0 && reach >= stage(blk, 0); --blk) {
       const int rows_b = (blk >= comb && comb < nb) ? (int)n : R;
       const int Mp = pad16(rows_b);
       const int64_t cnt = (int64_t)rows_b * d;
       const unsigned eg = (unsigned)((cnt + 255) / 256);
       // fc_1: dW1 += dh^T relu(n), db1 += colsum(dh); dn = (dh W1) * (n > 0)
-      BW(transpose_pad<false>(dh, d, rows_b, d, b.tA, Mp, s));
-      BW(transpose_pad<true>(b.nbuf[blk], d, rows_b, d, b.tB, Mp, s));
-      BW(gemm(b.tA, Mp, b.tB, nullptr, const_cast<float*>(grad.fc1_w[blk]), d, d, d, Mp, false, true, s));
-      BW(rowsum_acc(b.tA, Mp, d, const_cast<float*>(grad.fc1_b[blk]), s));
+      if (grad.fc1_w[blk] || grad.fc1_b[blk]) BW(transpose_pad<false>(dh, d, rows_b, d, b.tA, Mp, s));
+      if (grad.fc1_w[blk]) {
+        BW(transpose_pad<true>(b.nbuf[blk], d, rows_b, d, b.tB, Mp, s));
+        BW(gemm(b.tA, Mp, b.tB, nullptr, const_cast<float*>(grad.fc1_w[blk]), d, d, d, Mp, false, true, s));
+      }
+      if (grad.fc1_b[blk]) BW(rowsum_acc(b.tA, Mp, d, const_cast<float*>(grad.fc1_b[blk]), s));
+      if (reach < stage(blk, 1)) break;
       if (use_tc_gemm()) {   // the ReLU mask rides in the GEMM's epilogue
         BW(gemm_bf16x3_masked(dh, d, b.w1T[blk], d, b.T, d, rows_b, d, d, false, b.nbuf[blk], s));
       } else {
@@ -539,10 +561,13 @@ int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src
         PNR_LAUNCH_CHECK();
       }
       // fc_0: dW0 += dn^T relu(hpre), db0 += colsum(dn); dh += (dn W0) * (hpre > 0)
-      BW(transpose_pad<false>(b.T, d, rows_b, d, b.tA, Mp, s));
-      BW(transpose_pad<true>(b.hpre[blk], d, rows_b, d, b.tB, Mp, s));
-      BW(gemm(b.tA, Mp, b.tB, nullptr, const_cast<float*>(grad.fc0_w[blk]), d, d, d, Mp, false, true, s));
-      BW(rowsum_acc(b.tA, Mp, d, const_cast<float*>(grad.fc0_b[blk]), s));
+      if (grad.fc0_w[blk] || grad.fc0_b[blk]) BW(transpose_pad<false>(b.T, d, rows_b, d, b.tA, Mp, s));
+      if (grad.fc0_w[blk]) {
+        BW(transpose_pad<true>(b.hpre[blk], d, rows_b, d, b.tB, Mp, s));
+        BW(gemm(b.tA, Mp, b.tB, nullptr, const_cast<float*>(grad.fc0_w[blk]), d, d, d, Mp, false, true, s));
+      }
+      if (grad.fc0_b[blk]) BW(rowsum_acc(b.tA, Mp, d, const_cast<float*>(grad.fc0_b[blk]), s));
+      if (reach < stage(blk, 2)) break;
       if (use_tc_gemm()) {
         BW(gemm_bf16x3_masked(b.T, d, b.w0T[blk], d, dh, d, rows_b, d, d, true, b.hpre[blk], s));
       } else {
@@ -551,31 +576,36 @@ int field_backward(const PnrScene& sc, const PnrMlp& mlp, const PointSource& src
         PNR_LAUNCH_CHECK();
       }
       if (blk < comb) {   // x = x + lin_z[blk](latent): dWz += dh^T lat, dbz += colsum(dh), dlat += dh Wz
-        if (!lat_transposed) {
+        if (grad.lin_z_w[blk] && !lat_transposed) {
           BW(transpose_pad<false>(b.lat, L, R, L, b.latT, Rp, s));
           lat_transposed = true;
         }
-        BW(transpose_pad<false>(dh, d, R, d, b.tA, Rp, s));
-        BW(gemm(b.tA, Rp, b.latT, nullptr, const_cast<float*>(grad.lin_z_w[blk]), L, d, L, Rp, false, true, s));
-        BW(rowsum_acc(b.tA, Rp, d, const_cast<float*>(grad.lin_z_b[blk]), s));
-        BW(gemm(dh, d, b.wzT[blk], nullptr, b.dlat, L, R, L, d, false, true, s));
+        if (grad.lin_z_w[blk] || grad.lin_z_b[blk]) BW(transpose_pad<false>(dh, d, R, d, b.tA, Rp, s));
+        if (grad.lin_z_w[blk])
+          BW(gemm(b.tA, Rp, b.latT, nullptr, const_cast<float*>(grad.lin_z_w[blk]), L, d, L, Rp, false, true, s));
+        if (grad.lin_z_b[blk]) BW(rowsum_acc(b.tA, Rp, d, const_cast<float*>(grad.lin_z_b[blk]), s));
+        if (want_dlat) BW(gemm(dh, d, b.wzT[blk], nullptr, b.dlat, L, R, L, d, false, true, s));
       }
-      if (blk == comb && comb < nb && NS > 1) {   // the block's input was the mean over views
+      if (blk == comb && comb < nb && NS > 1 && reach > stage(blk, 2)) {   // the block's input was the mean over views
         k_view_mean_bwd<<<(unsigned)(((int64_t)R * d + 255) / 256), 256, 0, s>>>(dh, dh_other, n, NS, d);
         PNR_LAUNCH_CHECK();
         float* t = dh; dh = dh_other; dh_other = t;
       }
     }
     // lin_in: dW += dh^T feat (42 of the 48 padded columns), db += colsum(dh), dfeat = dh W_in
-    BW(transpose_pad<false>(dh, d, R, d, b.tA, Rp, s));
-    BW(transpose_pad<false>(b.feat, 48, R, 48, b.featT, Rp, s));
-    BW(gemm(b.tA, Rp, b.featT, nullptr, b.tmp_win, 48, d, 48, Rp, false, false, s));
-    k_add_cols<<<(d * mlp.d_in + 255) / 256, 256, 0, s>>>(const_cast<float*>(grad.lin_in_w), b.tmp_win, d, mlp.d_in, 48);
-    PNR_LAUNCH_CHECK();
-    BW(rowsum_acc(b.tA, Rp, d, const_cast<float*>(grad.lin_in_b), s));
+    if (grad.lin_in_w || grad.lin_in_b) BW(transpose_pad<false>(dh, d, R, d, b.tA, Rp, s));
+    if (grad.lin_in_w) {
+      BW(transpose_pad<false>(b.feat, 48, R, 48, b.featT, Rp, s));
+      BW(gemm(b.tA, Rp, b.featT, nullptr, b.tmp_win, 48, d, 48, Rp, false, false, s));
+      k_add_cols<<<(d * mlp.d_in + 255) / 256, 256, 0, s>>>(const_cast<float*>(grad.lin_in_w), b.tmp_win, d, mlp.d_in,
+                                                            48);
+      PNR_LAUNCH_CHECK();
+    }
+    if (grad.lin_in_b) BW(rowsum_acc(b.tA, Rp, d, const_cast<float*>(grad.lin_in_b), s));
+    if (!want_geom) continue;
     BW(gemm(dh, d, b.w_inT, nullptr, b.dfeat, 48, R, 48, d, false, false, s));
     float* cam_part = want_cam ? b.T : nullptr;    // [R][16]; T (R x d, d >= 16) is free again here
-    k_geom_bwd<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(sc, src, g0, n, b.dfeat, b.dlat,
+    k_geom_bwd<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(sc, src, g0, n, b.dfeat, want_dlat ? b.dlat : nullptr,
                                                                det ? nullptr : d_latent, d_xyz, d_dirs, cam_part);
     PNR_LAUNCH_CHECK();
     if (det && d_latent) BW(latent_scatter_fixed(sc, src, g0, n, b.dlat, d_latent, b.lat_fixed, b.m_bits, s));

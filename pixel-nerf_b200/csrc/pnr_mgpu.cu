@@ -325,11 +325,13 @@ int pnr_mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardG
                                       d_latent0_nhwc, nullptr, nullptr, B, stream0);
 }
 
-int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
-                                 const PnrShardCam* shard_cams, const PnrRenderCfg* cfg, const PnrRenderGrad* up0,
-                                 const PnrMlp* grad_coarse0, const PnrMlp* grad_fine0, float* d_latent0_nhwc,
-                                 float* d_rays0, const PnrCameraGrad* cam0, int64_t B, void* stream0) {
-  PNR_CHECK_ARG(h && shards && shard_grads && cfg && grad_coarse0, "NULL argument");
+// pnr_mgpu_render_backward_cam (sel = false) and pnr_mgpu_render_backward_sel (sel = true: NULL gradient structs /
+// members are frozen, NULL in the same places on every shard; the arenas hold only the wanted tensors, and may be empty)
+static int mgpu_render_backward(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
+                                const PnrShardCam* shard_cams, const PnrRenderCfg* cfg, const PnrRenderGrad* up0,
+                                const PnrMlp* grad_coarse0, const PnrMlp* grad_fine0, float* d_latent0_nhwc,
+                                float* d_rays0, const PnrCameraGrad* cam0, int64_t B, void* stream0, bool sel) {
+  PNR_CHECK_ARG(h && shards && shard_grads && cfg && (sel || grad_coarse0), "NULL argument");
   const PnrCameraGrad c0 = cam0 ? *cam0 : PnrCameraGrad{};
   const bool want_cam = c0.d_poses || c0.d_focal || c0.d_c;
   // shard i's camera buffers: those of cam0 that are wanted, at the same arena offsets on device i
@@ -372,15 +374,22 @@ int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrSh
     PNR_CHECK_ARG(sg.rays && sg.z_coarse && sg.workspace, "incomplete shard gradient (rays, z_coarse, workspace)");
     if (any_up && (i > 0 || SB > 1)) PNR_CHECK_ARG(sg.up_stage, "shard gradient needs an upstream staging buffer");
     if (i > 0) {
-      PNR_CHECK_ARG(sg0.arena && sg0.arena_count > 0, "shard gradient 0 needs device 0's gradient arena");
-      PNR_CHECK_ARG(sg.arena && sg.arena_count == sg0.arena_count, "shard gradient needs an arena of device 0's size");
-      PNR_CHECK_ARG(sg.grad_coarse && (!sh.mlp_fine || sg.grad_fine), "incomplete shard gradient (grad_coarse / grad_fine)");
+      PNR_CHECK_ARG((sg0.arena && sg0.arena_count > 0) || (sel && sg0.arena_count == 0),
+                    "shard gradient 0 needs device 0's gradient arena");
+      PNR_CHECK_ARG((sg.arena || sg0.arena_count == 0) && sg.arena_count == sg0.arena_count,
+                    "shard gradient needs an arena of device 0's size");
+      if (sel)
+        PNR_CHECK_ARG(!sg.grad_coarse == !grad_coarse0 && (!sh.mlp_fine || !sg.grad_fine == !grad_fine0),
+                      "shard gradient structs must be NULL where device 0's are");
+      else
+        PNR_CHECK_ARG(sg.grad_coarse && (!sh.mlp_fine || sg.grad_fine),
+                      "incomplete shard gradient (grad_coarse / grad_fine)");
       PNR_CHECK_ARG(same_layout(sg.grad_coarse, sg.arena, grad_coarse0, sg0.arena, sg0.arena_count) &&
                         same_layout(sh.mlp_fine ? sg.grad_fine : nullptr, sg.arena,
                                     sh.mlp_fine ? grad_fine0 : nullptr, sg0.arena, sg0.arena_count) &&
                         same_offset(sg.d_latent_nhwc, sg.arena, d_latent0_nhwc, sg0.arena, sg0.arena_count),
                     "shard gradient arena must have device 0's layout");
-      PNR_CHECK_ARG(h->peer_from_0[i] || sg.arena_stage0, "shard gradient needs a device-0 staging arena (no peer access)");
+      PNR_CHECK_ARG(h->peer_from_0[i] || sg.arena_stage0 || sg0.arena_count == 0, "shard gradient needs a device-0 staging arena (no peer access)");
       if (want_cam) {
         PNR_CHECK_ARG(shard_cams, "camera gradients need the per-shard camera buffers");
         const PnrCameraGrad ci = shard_cam(i);
@@ -426,7 +435,7 @@ int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrSh
       gi.*fields[k] = stage;
       stage += SB * Bi * w;
     }
-    if (i > 0) PNR_CUDA(cudaMemsetAsync(sg.arena, 0, (size_t)sg.arena_count * 4, s));
+    if (i > 0 && sg.arena_count > 0) PNR_CUDA(cudaMemsetAsync(sg.arena, 0, (size_t)sg.arena_count * 4, s));
     PnrRenderOut fwd{};
     fwd.z_coarse = const_cast<float*>(sg.z_coarse);
     fwd.z_fine = const_cast<float*>(sg.z_fine);
@@ -435,10 +444,10 @@ int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrSh
     const bool in_place = i == 0 && SB == 1;
     float* dr = d_rays0 ? (in_place ? d_rays0 : shard_cams[i].d_rays) : nullptr;
     const PnrCameraGrad ci = want_cam ? shard_cam(i) : PnrCameraGrad{};
-    int rc = pnr_render_backward_cam(sh.scene, sh.mlp_coarse, sh.mlp_fine, cfg, sg.rays, sh.noise, &fwd, &gi,
-                                     i == 0 ? grad_coarse0 : sg.grad_coarse, i == 0 ? grad_fine0 : sg.grad_fine,
-                                     i == 0 ? d_latent0_nhwc : sg.d_latent_nhwc, dr, want_cam ? &ci : nullptr, Bi,
-                                     sg.workspace, sg.workspace_bytes, s);
+    int rc = (sel ? pnr_render_backward_sel : pnr_render_backward_cam)(
+        sh.scene, sh.mlp_coarse, sh.mlp_fine, cfg, sg.rays, sh.noise, &fwd, &gi, i == 0 ? grad_coarse0 : sg.grad_coarse,
+        i == 0 ? grad_fine0 : sg.grad_fine, i == 0 ? d_latent0_nhwc : sg.d_latent_nhwc, dr, want_cam ? &ci : nullptr, Bi,
+        sg.workspace, sg.workspace_bytes, s);
     if (rc) return rc;
     // the reverse of the forward's ray staging: [SB][B_i][8] -> rows [a, b) of each object in d_rays0 [SB][B][8]
     if (dr && !in_place && (rc = copy_rows(d_rays0 + a * 8, B * 8, dr, Bi * 8, Bi * 8, SB, s))) return rc;
@@ -454,6 +463,7 @@ int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrSh
     if (b - a <= 0) continue;
     const PnrShardGrad& sg = shard_grads[i];
     PNR_CUDA(cudaStreamWaitEvent(s0, h->done[i], 0));
+    if (sg.arena_count == 0) continue;                           // nothing in the arenas (e.g. ray gradients only)
     if (h->peer_from_0[i]) {
       src.push_back(sg.arena);                                   // read over NVLink by the reduction kernel
     } else {
@@ -472,6 +482,22 @@ int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrSh
     PNR_CUDA(cudaStreamWaitEvent(streams[i], h->reduced, 0));
   }
   return PNR_OK;
+}
+
+int pnr_mgpu_render_backward_cam(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
+                                 const PnrShardCam* shard_cams, const PnrRenderCfg* cfg, const PnrRenderGrad* up0,
+                                 const PnrMlp* grad_coarse0, const PnrMlp* grad_fine0, float* d_latent0_nhwc,
+                                 float* d_rays0, const PnrCameraGrad* cam0, int64_t B, void* stream0) {
+  return mgpu_render_backward(h, shards, shard_grads, shard_cams, cfg, up0, grad_coarse0, grad_fine0, d_latent0_nhwc,
+                              d_rays0, cam0, B, stream0, false);
+}
+
+int pnr_mgpu_render_backward_sel(PnrMgpu* h, const PnrShard* shards, const PnrShardGrad* shard_grads,
+                                 const PnrShardCam* shard_cams, const PnrRenderCfg* cfg, const PnrRenderGrad* up0,
+                                 const PnrMlp* grad_coarse0, const PnrMlp* grad_fine0, float* d_latent0_nhwc,
+                                 float* d_rays0, const PnrCameraGrad* cam0, int64_t B, void* stream0) {
+  return mgpu_render_backward(h, shards, shard_grads, shard_cams, cfg, up0, grad_coarse0, grad_fine0, d_latent0_nhwc,
+                              d_rays0, cam0, B, stream0, true);
 }
 
 }  // extern "C"

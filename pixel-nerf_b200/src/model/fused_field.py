@@ -9,7 +9,10 @@ The autograd node takes the sample positions, the view directions, the latent, t
 renderer (sample depths, rays), `d_latent` into the encoder trunk, the camera gradients to the poses / focal / c given
 to encode() and the weight gradients into the optimiser, exactly where the reference's graph has them
 (train/train.py:199-215, models.py:112-212).  Only the gradients autograd asks for are computed; without view-direction
-or camera gradients the backward is `pnr_field_backward`, otherwise `pnr_field_backward_cam`.
+or camera gradients the backward is `pnr_field_backward`, otherwise `pnr_field_backward_cam`.  With some MLP
+parameters frozen (`requires_grad=False`) it is `pnr_field_backward_sel`: the frozen tensors' gradients are neither
+allocated nor computed (no weight-gradient GEMM, transposes or bias sum, and no input-gradient chain below the lowest
+trainable layer unless an input gradient is wanted) and come back as None; the others are bit-equal to the full call's.
 """
 import torch
 
@@ -35,10 +38,11 @@ class _FusedField(torch.autograd.Function):
         m = mf if use_fine else mc
         dev = xyz.device
         names = [k for k, _ in mlp.named_parameters()]
+        wanted = ctx.needs_input_grad[8:]
         grads = {k: torch.zeros_like(p, dtype=torch.float32, memory_format=torch.contiguous_format)
-                 for k, p in mlp.named_parameters()}
+                 for (k, p), w in zip(mlp.named_parameters(), wanted) if w}
         gstruct = pn.make_mlp_struct(grads, mlp.d_in, mlp.d_latent, mlp.d_hidden, mlp.d_out, mlp.n_blocks,
-                                     mlp.combine_layer)
+                                     mlp.combine_layer) if grads else None
         V, C, Hl, Wl = net.encoder.latent.shape
         want_latent = ctx.needs_input_grad[4]
         d_latent = torch.zeros(V, Hl, Wl, C, dtype=torch.float32, device=dev) if want_latent else None
@@ -53,7 +57,12 @@ class _FusedField(torch.autograd.Function):
         nbytes = L.pnr_field_backward_workspace_bytes(scene, m, B)
         ws = pn.workspace(dev, nbytes)
         with torch.cuda.device(dev):
-            if d_dirs is None and cam is None:
+            if not all(wanted):      # part of the MLP is frozen
+                pn.check(L.pnr_field_backward_sel(scene, m, pn.dptr(xyz_c, "xyz"), pn.dptr(dirs_c, "viewdirs"),
+                                                  pn.dptr(d_out_c, "d_out"), gstruct, pn.dptr(d_latent),
+                                                  pn.dptr(d_xyz), pn.dptr(d_dirs), cam, B, ws.data_ptr(), ws.numel(),
+                                                  pn.stream_ptr(dev)))
+            elif d_dirs is None and cam is None:
                 pn.check(L.pnr_field_backward(scene, m, pn.dptr(xyz_c, "xyz"), pn.dptr(dirs_c, "viewdirs"),
                                               pn.dptr(d_out_c, "d_out"), gstruct, pn.dptr(d_latent), pn.dptr(d_xyz),
                                               B, ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
@@ -64,7 +73,7 @@ class _FusedField(torch.autograd.Function):
                                                   pn.stream_ptr(dev)))
         g_latent = d_latent.permute(0, 3, 1, 2) if want_latent else None
         g_dirs = d_dirs.reshape(viewdirs.shape) if d_dirs is not None else None
-        return (None, None, d_xyz, g_dirs, g_latent) + d_cam + tuple(grads[k] for k in names)
+        return (None, None, d_xyz, g_dirs, g_latent) + d_cam + tuple(grads.get(k) for k in names)
 
 
 def fused_field(net, xyz, coarse, viewdirs):

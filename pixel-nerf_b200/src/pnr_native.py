@@ -119,6 +119,10 @@ def declare(L):
                                           P(PnrRenderOut), P(PnrRenderGrad), P(PnrMlp), P(PnrMlp), vp, vp,
                                           P(PnrCameraGrad), i64, vp, sz, vp]
     L.pnr_render_backward_cam.restype = C.c_int
+    L.pnr_field_backward_sel.argtypes = L.pnr_field_backward_cam.argtypes
+    L.pnr_field_backward_sel.restype = C.c_int
+    L.pnr_render_backward_sel.argtypes = L.pnr_render_backward_cam.argtypes
+    L.pnr_render_backward_sel.restype = C.c_int
     L.pnr_gen_rays_backward.argtypes = [vp, vp, i64, i32, i32, f32, f32, f32, f32, i64, i64, vp, vp]
     L.pnr_gen_rays_backward.restype = C.c_int
     L.pnr_composite_backward.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, i32, vp]
@@ -149,9 +153,11 @@ def declare(L):
         L.pnr_mgpu_render_backward_cam.argtypes = [vp, P(PnrShard), P(PnrShardGrad), P(PnrShardCam), P(PnrRenderCfg),
                                                    P(PnrRenderGrad), P(PnrMlp), P(PnrMlp), vp, vp, P(PnrCameraGrad),
                                                    i64, vp]
+        L.pnr_mgpu_render_backward_sel.argtypes = L.pnr_mgpu_render_backward_cam.argtypes
         L.pnr_sum_into.argtypes = [vp, P(vp), i32, i64, vp]
         for name in ("pnr_mgpu_create", "pnr_mgpu_destroy", "pnr_mgpu_broadcast", "pnr_mgpu_render",
-                     "pnr_mgpu_render_backward", "pnr_mgpu_render_backward_cam", "pnr_sum_into"):
+                     "pnr_mgpu_render_backward", "pnr_mgpu_render_backward_cam", "pnr_mgpu_render_backward_sel",
+                     "pnr_sum_into"):
             getattr(L, name).restype = C.c_int
     if hasattr(L, "pnr_grid_points"):     # (the host-emulator build of tests/cuda_emu has no mesh extraction)
         f64 = C.c_double
@@ -389,22 +395,19 @@ def workspace(device, nbytes):
 # Struct builders
 # ------------------------------------------------------------------------------------------
 def make_mlp_struct(sd, d_in, d_latent, d_hidden, d_out, n_blocks, combine_layer, packed=None):
-    """sd: dict name -> contiguous fp32 CUDA tensor with ResnetFC state_dict keys."""
+    """sd: dict name -> contiguous fp32 CUDA tensor with ResnetFC state_dict keys.  A key missing from sd leaves its
+    pointer NULL (a frozen tensor of a gradient struct for the _sel backward entry points)."""
     m = PnrMlp()
     m.d_in, m.d_latent, m.d_hidden, m.d_out = d_in, d_latent, d_hidden, d_out
     m.n_blocks, m.combine_layer = n_blocks, combine_layer
-    m.lin_in_w, m.lin_in_b = dptr(sd["lin_in.weight"]), dptr(sd["lin_in.bias"])
-    m.lin_out_w, m.lin_out_b = dptr(sd["lin_out.weight"]), dptr(sd["lin_out.bias"])
+    p = lambda k: dptr(sd.get(k), k)
+    m.lin_in_w, m.lin_in_b = p("lin_in.weight"), p("lin_in.bias")
+    m.lin_out_w, m.lin_out_b = p("lin_out.weight"), p("lin_out.bias")
     for i in range(n_blocks):
-        m.fc0_w[i] = sd[f"blocks.{i}.fc_0.weight"].data_ptr()
-        m.fc0_b[i] = sd[f"blocks.{i}.fc_0.bias"].data_ptr()
-        m.fc1_w[i] = sd[f"blocks.{i}.fc_1.weight"].data_ptr()
-        m.fc1_b[i] = sd[f"blocks.{i}.fc_1.bias"].data_ptr()
-        dptr(sd[f"blocks.{i}.fc_0.weight"]), dptr(sd[f"blocks.{i}.fc_1.weight"])
+        m.fc0_w[i], m.fc0_b[i] = p(f"blocks.{i}.fc_0.weight"), p(f"blocks.{i}.fc_0.bias")
+        m.fc1_w[i], m.fc1_b[i] = p(f"blocks.{i}.fc_1.weight"), p(f"blocks.{i}.fc_1.bias")
     for i in range(min(combine_layer, n_blocks)):
-        m.lin_z_w[i] = sd[f"lin_z.{i}.weight"].data_ptr()
-        m.lin_z_b[i] = sd[f"lin_z.{i}.bias"].data_ptr()
-        dptr(sd[f"lin_z.{i}.weight"])
+        m.lin_z_w[i], m.lin_z_b[i] = p(f"lin_z.{i}.weight"), p(f"lin_z.{i}.bias")
     if packed is not None:
         m.packed = C.c_void_p(packed.data_ptr())
         m.packed_bytes = packed.numel() * packed.element_size()

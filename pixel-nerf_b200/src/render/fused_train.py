@@ -27,6 +27,16 @@ pnr_mgpu_render_backward_cam, whose camera gradients sit in the same per-shard a
 
 Both nodes set up their forward call with render/fused_call.py, take the same inputs after their leading arguments
 (`_apply`), and lay out their gradients in one zeroed buffer per device (`_grad_arena`).
+
+Frozen MLP parameters (`requires_grad=False`: pose refinement, fine-tuning only some layers) cost nothing in the
+backward.  Each node reads per parameter whether autograd wants its gradient; the arena then holds only the
+wanted ones, the frozen ones stay NULL in the gradient structs and get None, and the call goes to the `_sel` entry
+point (`pnr_render_backward_sel` / `pnr_mgpu_render_backward_sel`).  That skips a frozen tensor's weight-gradient GEMM,
+its transposes and its bias sum, the input-gradient chain below the lowest trainable layer when no input gradient is
+wanted, the latent and geometry backward when none of latent, rays or cameras is wanted, and a whole pass with nothing
+to train or differentiate.  The wanted gradients are bit-equal to the full call's.  With every parameter trainable the
+calls are exactly the ones described above, and so is the sharded node's call for a wholly frozen network (ray and
+camera gradients only): that one still runs the full backward and drops the weight gradients.
 """
 import ctypes as C
 
@@ -63,29 +73,33 @@ def _upstream(names, grads, dev):
     return ug, up
 
 
-def _grad_arena(net, fine, needs, dev):
-    """One zeroed fp32 buffer on `dev` holding every parameter gradient of the MLPs the call runs and, where `needs`
-    (latent, poses, focal, c: four bools) asks, the channels-last latent gradient and the camera gradients, so that one
-    kernel reduces a shard's whole gradient.  Every device gets the same layout.  -> (flat, [parameter gradient views in
-    the order of the node's inputs], (PnrMlp coarse, PnrMlp fine or None), latent view or None, (d_poses, d_focal, d_c)
-    views or None, PnrCameraGrad or None when no camera gradient is asked for)."""
+def _grad_arena(net, fine, needs, wanted, dev):
+    """One zeroed fp32 buffer on `dev` holding the gradient of every parameter of the MLPs the call runs that `wanted`
+    (one bool per parameter, in the node's input order) asks for and, where `needs` (latent, poses, focal, c: four bools)
+    asks, the channels-last latent gradient and the camera gradients, so that one kernel reduces a shard's whole
+    gradient.  Every device gets the same layout.  -> (flat, [parameter gradient views in the order of the node's inputs,
+    None where not wanted], (PnrMlp coarse, PnrMlp fine) with frozen tensors NULL, or None for a wholly frozen or absent
+    MLP, latent view or None, (d_poses, d_focal, d_c) views or None, PnrCameraGrad or None when no camera gradient is
+    asked for)."""
     mlps = _mlps(net, fine)
     V, Cc, Hl, Wl = net.encoder.latent.shape
     lat_shape = (V, Hl, Wl, Cc) if needs[0] else None
     cam_shapes = [t.shape if need else None for t, need in zip((net.poses, net.focal, net.c), needs[1:])]
-    sizes = [p.numel() for mlp in mlps for p in mlp.parameters()]
+    params = [p for mlp in mlps for p in mlp.parameters()]
+    sizes = [p.numel() for p, w in zip(params, wanted) if w]
     lat_n = 0 if lat_shape is None else torch.Size(lat_shape).numel()
     cam_n = [0 if sh is None else torch.Size(sh).numel() for sh in cam_shapes]
     flat = torch.zeros(sum(sizes) + lat_n + sum(cam_n), dtype=torch.float32, device=dev)
-    grads, structs, off = [], [], 0
+    grads, structs, off, wanted = [], [], 0, iter(wanted)
     for mlp in mlps:
         g = {}
         for k, p in mlp.named_parameters():
-            g[k] = flat[off:off + p.numel()].view(p.shape)
-            off += p.numel()
-        grads += g.values()
+            if next(wanted):
+                g[k] = flat[off:off + p.numel()].view(p.shape)
+                off += p.numel()
+            grads.append(g.get(k))
         structs.append(pn.make_mlp_struct(g, mlp.d_in, mlp.d_latent, mlp.d_hidden, mlp.d_out, mlp.n_blocks,
-                                          mlp.combine_layer))
+                                          mlp.combine_layer) if g else None)
     lat = flat[off:off + lat_n].view(lat_shape) if lat_shape is not None else None
     off += lat_n
     cams = []
@@ -94,6 +108,10 @@ def _grad_arena(net, fine, needs, dev):
         off += k
     cam = pn.PnrCameraGrad(*(pn.dptr(t) for t in cams)) if any(t is not None for t in cams) else None
     return flat, grads, (structs[0], structs[1] if len(structs) > 1 else None), lat, tuple(cams), cam
+
+
+def _mlp_ref(struct):
+    return C.byref(struct) if struct is not None else None
 
 
 def _apply(node, lead, net, renderer, rays, want_weights, noise_in):
@@ -136,7 +154,8 @@ class _FusedRender(torch.autograd.Function):
         SB, B, _ = rays.shape
         ug, up = _upstream(ctx.names, grads, dev)
         scene, mc, mf, keep = model._scene_struct(want_fine=fine)
-        flat, pgrads, (gc, gf), d_latent, d_cam, cam = _grad_arena(model, fine, ctx.needs_input_grad[5:9], dev)
+        wanted = ctx.needs_input_grad[9:]
+        flat, pgrads, (gc, gf), d_latent, d_cam, cam = _grad_arena(model, fine, ctx.needs_input_grad[5:9], wanted, dev)
         noise = fc.bind_noise(renderer._lin_steps(Kc, dev), ctx.noise)
         fwd = fc.bind_outputs(ctx.fwd)
         L = pn.lib()
@@ -144,7 +163,11 @@ class _FusedRender(torch.autograd.Function):
         pn.sync_deterministic()
         ws = pn.workspace(dev, L.pnr_render_backward_workspace_bytes(scene, mc, mf, ctx.cfg, B))
         with torch.cuda.device(dev):
-            if d_rays is None and cam is None:
+            if not all(wanted):      # part of the network is frozen
+                pn.check(L.pnr_render_backward_sel(scene, mc, mf, ctx.cfg, pn.dptr(rays, "rays"), noise, fwd, ug,
+                                                   _mlp_ref(gc), _mlp_ref(gf), pn.dptr(d_latent), pn.dptr(d_rays), cam,
+                                                   B, ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
+            elif d_rays is None and cam is None:
                 pn.check(L.pnr_render_backward_ex(scene, mc, mf, ctx.cfg, pn.dptr(rays, "rays"), noise, fwd, ug, gc, gf,
                                                   pn.dptr(d_latent), B, ws.data_ptr(), ws.numel(), pn.stream_ptr(dev)))
             else:
@@ -197,8 +220,13 @@ class _ShardedFusedRender(torch.autograd.Function):
         dev0 = torch.device("cuda", gpus[0])
         L = pn.lib()
         ug, up = _upstream(ctx.names, grads, dev0)
-        needs = ctx.needs_input_grad[4:8]
-        flat0, pgrads, (gc0, gf0), d_lat0, d_cam0, cam0 = _grad_arena(net, fine, needs, dev0)
+        needs, wanted = ctx.needs_input_grad[4:8], ctx.needs_input_grad[8:]
+        # A partly frozen network takes the selective driver.  A wholly frozen one (sharded pose refinement) keeps the
+        # driver call it has always made, pnr_mgpu_render_backward_cam over full arenas, whose weight gradients are
+        # then dropped.
+        sel = any(wanted) and not all(wanted)
+        layout = wanted if sel else (True,) * len(wanted)
+        flat0, pgrads, (gc0, gf0), d_lat0, d_cam0, cam0 = _grad_arena(net, fine, needs, layout, dev0)
         want_rays = ctx.needs_input_grad[3]
         d_rays0 = torch.empty(SB, B, 8, dtype=torch.float32, device=dev0) if want_rays else None
         scs = (pn.PnrShardCam * n)()
@@ -238,10 +266,10 @@ class _ShardedFusedRender(torch.autograd.Function):
                 if i == 0:
                     sg.arena, sg.arena_count = pn.dptr(flat0), flat0.numel()
                     continue
-                flat, _, (gc, gf), d_lat, _, cam = _grad_arena(net, fine, needs, dev)
+                flat, _, (gc, gf), d_lat, _, cam = _grad_arena(net, fine, needs, layout, dev)
                 if cam is not None:
                     scs[i].cam = cam
-                sg.grad_coarse = C.pointer(gc)
+                sg.grad_coarse = C.pointer(gc) if gc is not None else None
                 sg.grad_fine = C.pointer(gf) if gf is not None else None
                 sg.d_latent_nhwc = pn.dptr(d_lat)
                 sg.arena, sg.arena_count = pn.dptr(flat), flat.numel()
@@ -252,7 +280,11 @@ class _ShardedFusedRender(torch.autograd.Function):
                 keep.append(stage0)
         keep.append(wss)
         with torch.cuda.device(dev0):
-            if d_rays0 is None and cam0 is None:
+            if sel:
+                pn.check(L.pnr_mgpu_render_backward_sel(h, ctx.shards, sgs, scs, ctx.cfg, ug, _mlp_ref(gc0),
+                                                        _mlp_ref(gf0), pn.dptr(d_lat0), pn.dptr(d_rays0), cam0, B,
+                                                        pn.stream_ptr(dev0)))
+            elif d_rays0 is None and cam0 is None:
                 pn.check(L.pnr_mgpu_render_backward(h, ctx.shards, sgs, ctx.cfg, ug, gc0, gf0, pn.dptr(d_lat0), B,
                                                     pn.stream_ptr(dev0)))
             else:
@@ -262,7 +294,7 @@ class _ShardedFusedRender(torch.autograd.Function):
         sharded._keep_bwd = keep     # (the driver also orders every shard stream after the reduction)
         g_latent = d_lat0.permute(0, 3, 1, 2) if d_lat0 is not None else None
         g_rays = d_rays0.to(ctx.rays_device) if d_rays0 is not None else None
-        return (None, None, None, g_rays, g_latent) + d_cam0 + tuple(pgrads)
+        return (None, None, None, g_rays, g_latent) + d_cam0 + tuple(g if w else None for g, w in zip(pgrads, wanted))
 
 
 def sharded_render_train(sharded, rays, want_weights, noise_in=None):

@@ -23,8 +23,8 @@
 //  * 256 threads = two warpgroups (geometry, wgmma, epilogues, ray finishing), so ptxas may give each thread 255
 //    registers: the 160 accumulator registers plus addressing fit, and each step's 9 or 12 wgmma issue back to back
 //    as one commit group.  There is no weight-stream warp: each warpgroup has its own 4-slot ring of the 8 KB halves
-//    of the pre-swizzled 16 KB weight tiles that it multiplies, which its first thread refills (cp.async.bulk in
-//    consumption order, mbarrier full/empty) whenever the warpgroup releases a step's slots (struct Ring).
+//    of the pre-swizzled 16 KB weight tiles that it multiplies, which the last of its warps to release a step's slots
+//    refills at once (cp.async.bulk in consumption order onto FULL mbarriers; struct Ring).
 //    tests/test_tc_codegen.py guards the register budget.
 //  * k_field_tc_fast (PNR_ENGINE_TC_FAST) is the same body with FAST = true: one tensor pass per step, D += Ahi*Whi
 //    with fp32 accumulation.  It loads only the W_hi tile of each step (the W_lo slot of the ring stays idle) and never
@@ -62,6 +62,8 @@ constexpr int AH_BYTES = 2 * A_CHUNK_BYTES;  // relu(H_c): 128 hidden features
 constexpr int SLOTS_LIN_IN = 8;
 constexpr int SLOTS_BLOCK = 128;         // fc_0 and fc_1 of one ResNet block, interleaved by hidden chunk
 constexpr int SLOTS_TOTAL = SLOTS_LIN_IN + 5 * SLOTS_BLOCK;   // 648
+constexpr int SLOTS_HEAD = SLOTS_LIN_IN + 3 * SLOTS_BLOCK;    // lin_in + blocks 0-2, run once per view
+constexpr int SLOTS_TAIL = 2 * SLOTS_BLOCK;                   // blocks 3-4, run once per tile
 constexpr int HEADER_BYTES = 256;
 
 // shared memory map (offsets from the 1024-aligned base)
@@ -72,10 +74,9 @@ constexpr int SM_GEO = SM_B + NSLOTS * SLOT_BYTES;      // [64][8] words: 4 tap 
 constexpr int SM_PART = SM_A;                           // lin_out partials [64][2][4] floats alias A chunk 0 (free at tile end)
 constexpr int SM_BAR = SM_GEO + ROWS * 8 * 4;          // [2][BAR_COUNT]: the mbarriers of each warpgroup's ring
 constexpr int BAR_FULL = 0;                             // [NSLOTS]
-constexpr int BAR_EMPTY = BAR_FULL + NSLOTS;            // [NSLOTS]
-constexpr int BAR_COUNT = BAR_EMPTY + NSLOTS;
+constexpr int BAR_COUNT = BAR_FULL + NSLOTS;
 constexpr int SM_NLIST = SM_BAR + 2 * BAR_COUNT * 8;    // fused render: number of rays this CTA completed in the current pass
-constexpr int SM_FEED = SM_NLIST + 16;                  // struct Feed [2]: the weight-slot cursor of each warpgroup's ring
+constexpr int SM_FEED = SM_NLIST + 16;                  // struct Feed [2]: the refill cursor and release counts of each ring
 constexpr int FEED_BYTES = 128;
 constexpr int SM_PROF = SM_FEED + 2 * FEED_BYTES;       // phase counters of the profile build: [2][PH_COUNT] u64
 #ifdef PNR_TC_PROFILE
@@ -135,15 +136,17 @@ enum { MODE_GATHER = 0, MODE_BIAS_WB = 1, MODE_COMBINE = 2, MODE_OUT = 3 };
 
 // Phase profile (built with -DPNR_TC_PROFILE into lib/libpnr_sm90_prof.so, scripts/tc_phase_profile.py): the first
 // thread of each warpgroup adds the clock64() time it spends in each phase to a shared-memory counter and, at kernel
-// end, to the 8 counters that pnr_tc_counters returns.  The phases are disjoint; the rest of PH_TOTAL is wgmma issue,
-// the epilogue arithmetic and the refill's cursor walk.  The hooks are macros that the production build expands to
-// nothing, so its kernels are the same instructions with or without them (tests/test_tc_profile.py).
+// end, to the 8 counters that pnr_tc_counters returns.  The exception is PH_REFILL: the time spent issuing the ring's
+// refills, counted on whichever lane 0 releases a step last and so refills (struct Ring); a ring's refills never
+// overlap, so that plain add does not race.  The phases of the first thread are disjoint; the rest of PH_TOTAL is
+// wgmma issue and the epilogue arithmetic.  The hooks are macros that the production build expands to nothing, so its
+// kernels are the same instructions with or without them (tests/test_tc_profile.py).
 #ifdef PNR_TC_PROFILE
 extern __shared__ __align__(1024) uint8_t smem[];
-enum { PH_FULL, PH_EMPTY, PH_WGMMA_WAIT, PH_SYNC, PH_GATHER, PH_GEOM, PH_FLUSH, PH_TOTAL, PH_COUNT };
-__device__ __forceinline__ void prof_add(int ph, long long t0) {
+enum { PH_FULL, PH_REFILL, PH_WGMMA_WAIT, PH_SYNC, PH_GATHER, PH_GEOM, PH_FLUSH, PH_TOTAL, PH_COUNT };
+__device__ __forceinline__ void prof_add(int ph, long long t0, bool any_thread = false) {
   const long long dt = clock64() - t0;
-  if ((threadIdx.x & 127) == 0)
+  if (any_thread || (threadIdx.x & 127) == 0)
     reinterpret_cast<unsigned long long*>(smem + SM_PROF)[(threadIdx.x >> 7) * PH_COUNT + ph] += (unsigned long long)dt;
 }
 __device__ __forceinline__ void prof_finish(int* status, long long t_kernel) {
@@ -156,6 +159,7 @@ __device__ __forceinline__ void prof_finish(int* status, long long t_kernel) {
 #define PROF_BEGIN(t) long long t = clock64()
 #define PROF_RESTART(t) t = clock64()
 #define PROF_END(ph, t) prof_add(ph, t)
+#define PROF_END_ANY(ph, t) prof_add(ph, t, true)
 // before the kernel's first __syncthreads
 #define PROF_INIT() \
   if (threadIdx.x < 2 * PH_COUNT) reinterpret_cast<unsigned long long*>(smem + SM_PROF)[threadIdx.x] = 0
@@ -164,6 +168,7 @@ __device__ __forceinline__ void prof_finish(int* status, long long t_kernel) {
 #define PROF_BEGIN(t)
 #define PROF_RESTART(t)
 #define PROF_END(ph, t)
+#define PROF_END_ANY(ph, t)
 #define PROF_INIT()
 #define PROF_FINISH(status, t)
 #endif
@@ -214,82 +219,94 @@ __device__ __forceinline__ uint32_t swz(int m, int k) {
 extern __shared__ __align__(1024) uint8_t smem[];
 
 // The weight-slot sequence of one CTA, in consumption order: per pass, per tile of its pair, NS x (lin_in + blocks
-// 0-2: slots [0, 392) of the pass's weight image) then blocks 3-4 (slots [392, 648)).  Each warpgroup's producer
-// thread walks it one slot at a time with its own cursor; the cursors live in shared memory so that no register is
-// held for them across the MMA loops.
+// 0-2: slots [0, SLOTS_HEAD) of the pass's weight image) then blocks 3-4 (slots [SLOTS_HEAD, SLOTS_TOTAL)), i.e. runs
+// of consecutive slots.  Each ring walks it one step (two slots: W_hi, W_lo of one tile) per refill.  The cursor lives
+// in shared memory so that no register is held for it across the MMA loops, and it keeps the next step's source
+// address and the steps left in its run, so that a refill inside a run reads two words and writes them back; only the
+// refill that ends a run walks on to the next view, tile or pass.
 struct Feed {
-  const uint8_t* slots[2];   // first slot of each pass's weight image
+  const uint8_t* src;        // this warpgroup's half of the next step's W_hi slot; nullptr: the sequence is done
+  uint64_t keep;             // createpolicy evict_last for the weight images
+  int left;                  // steps left in the current run
+  uint32_t released[2];      // warp releases of the steps that use ring slots 0-1 / 2-3 (never reset: see Ring)
+  const uint8_t* slots[2];   // this warpgroup's half of the first slot of each pass's weight image
   int64_t n_tiles[2];
-  int64_t tile;              // tile of the next slot
+  int64_t tile;              // tile of the current run
   int npass, NS, pair, n_pairs;
-  int ps, v, i;              // pass (npass: sequence done), view (NS: the blocks 3-4 run), slot within the run
-  __device__ __forceinline__ void skip_empty_passes() {
+  int ps, v;                 // pass (npass: sequence done), view of the current run (NS: the blocks 3-4 run)
+  __device__ __forceinline__ void begin_run() {
     while (ps < npass && tile >= n_tiles[ps]) {
       ++ps;
       tile = pair;
     }
+    const bool head = v < NS;
+    src = ps < npass ? slots[ps] + (head ? 0 : (size_t)SLOTS_HEAD * SLOT_BYTES) : nullptr;
+    left = (head ? SLOTS_HEAD : SLOTS_TAIL) / 2;
+  }
+  __device__ __forceinline__ void next_run() {
+    if (++v > NS) {
+      v = 0;
+      tile += n_pairs;
+    }
+    begin_run();
   }
 };
 static_assert(sizeof(Feed) <= FEED_BYTES, "Feed does not fit its shared-memory slot");
+static_assert(SLOTS_HEAD % 2 == 0 && SLOTS_TAIL % 2 == 0, "a step's two slots lie in one run");
 static_assert(SM_PROF <= SMEM_BYTES, "the two rings' barriers and cursors fit under the block limit");
 __device__ __forceinline__ Feed& feed(int wg) { return *reinterpret_cast<Feed*>(smem + SM_FEED + wg * FEED_BYTES); }
 
-// Producer of warpgroup wg's ring (thread 128 wg only): load the warpgroup's halves of the two slots of the step whose
-// first slot has sequence number n, once the halves' previous contents (sequence numbers n - 4, n - 3) are released by
-// the warpgroup's 4 warps.  The single-pass engine loads the W_hi slot only (even sequence numbers: the weight image
-// stores every tile as hi, lo) and steps the cursor over W_lo.
+__device__ __forceinline__ uint32_t atom_add_acq_rel(uint32_t saddr, uint32_t v) {
+  uint32_t old;
+  asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(saddr), "r"(v) : "memory");
+  return old;
+}
+
+// Refill of warpgroup wg's ring: load the warpgroup's halves of the next step of its Feed into ring slots n % 4 and
+// n % 4 + 1 (n: sequence number of the step's first slot) and advance the cursor by one step.  The single-pass engine
+// loads the W_hi slot only (the weight image stores every tile as hi, lo) and steps over W_lo.
 template <bool FAST>
-__device__ __forceinline__ void feed_step(uint32_t bar_base, uint32_t b_base, uint32_t n, int wg, int* status) {
+__device__ __forceinline__ void refill(uint32_t bar_base, uint32_t b_base, uint32_t n, int wg) {
   Feed& f = feed(wg);
-#pragma unroll 1
-  for (uint32_t s = n; s < n + 2; ++s) {
-    if (f.ps >= f.npass) return;
-    const bool load = !FAST || s % 2 == 0;
-    const uint32_t sl = s % NSLOTS, ph = (s / NSLOTS) & 1;
-    PROF_BEGIN(t0);
-    if (load) mbar_wait(bar_base + (BAR_EMPTY + sl) * 8, ph ^ 1, status, 410 + 4 * wg + sl);
-    PROF_END(PH_EMPTY, t0);
-    const uint32_t full = bar_base + (BAR_FULL + sl) * 8;
-    const bool head = f.v < f.NS;   // lin_in + blocks 0-2 of view v, else blocks 3-4
-    if (load) {
-      // every CTA streams the same 2 x 10 MB of weight images; keep them in L2 ahead of the projected maps that the
-      // gather streams past them (evict_first, stage_gather)
-      uint64_t keep;
-      asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(keep));
-      mbar_expect_tx(full, HALF_SLOT_BYTES);
-      bulk_g2s_hint(b_base + sl * SLOT_BYTES,
-                    f.slots[f.ps] + (size_t)((head ? 0 : SLOTS_LIN_IN + 3 * SLOTS_BLOCK) + f.i) * SLOT_BYTES +
-                        wg * HALF_SLOT_BYTES,
-                    HALF_SLOT_BYTES, full, keep);
-    }
-    if (++f.i == (head ? SLOTS_LIN_IN + 3 * SLOTS_BLOCK : 2 * SLOTS_BLOCK)) {
-      f.i = 0;
-      if (++f.v > f.NS) {
-        f.v = 0;
-        f.tile += f.n_pairs;
-        f.skip_empty_passes();
-      }
-    }
+  const uint8_t* src = f.src;
+  if (src == nullptr) return;
+  // every CTA streams the same 2 x 10 MB of weight images; keep them in L2 ahead of the projected maps that the
+  // gather streams past them (evict_first, stage_gather)
+  const uint64_t keep = f.keep;
+  const uint32_t sl = n % NSLOTS;
+#pragma unroll
+  for (uint32_t k = 0; k < (FAST ? 1u : 2u); ++k) {
+    const uint32_t full = bar_base + (BAR_FULL + sl + k) * 8;
+    mbar_expect_tx(full, HALF_SLOT_BYTES);
+    bulk_g2s_hint(b_base + (sl + k) * SLOT_BYTES, src + k * SLOT_BYTES, HALF_SLOT_BYTES, full, keep);
   }
+  const int left = f.left - 1;
+  f.left = left;
+  if (left == 0)
+    f.next_run();
+  else
+    f.src = src + 2 * SLOT_BYTES;
 }
 
 // Weight rings: one per warpgroup.  Warpgroup g multiplies only rows [64g, 64g+64) of every 128-row weight tile, the
 // contiguous 8 KB at byte 8192 g of each 16 KB slot, so each warpgroup streams its own halves of the 4 slots
-// with its own FULL / EMPTY mbarriers and its own Feed cursor; the two rings share nothing.  The halves are filled in
+// with its own FULL mbarriers, release counts and Feed cursor; the two rings share nothing.  The halves are filled in
 // exactly the order the warpgroup uses them; every step takes two consecutive slots (W_hi, W_lo of one 128-row x 64-k
-// tile).  A step's halves are released once the wgmma that read them have completed (one step later: wait_group 1, or
-// at the drain that ends an MMA run), and the release refills them with the step two ahead: the warpgroup's first
-// thread (0 or 128) waits until the warpgroup's 4 warps have released them (EMPTY), then issues the cp.async.bulk.
-// Steps 0 and 1 are loaded at kernel start.  A warpgroup never waits for the other one's refill, so the two may drift
-// apart by up to a step between two workers_sync, which staggers their use of the tensor pipe and of L2.
-// This EMPTY wait cannot deadlock: it depends only on the waiting thread's own warpgroup.  When thread 128g waits in
-// the release of step s, it has released s itself; warps 1-3 of its warpgroup release s in their `issued` of step
-// s+1 or their drain after step s, with no workers_sync in between (every MMA run ends with a drain before the next
-// workers_sync).  To get there they need only FULL of step s+1, whose load thread 128g issued at the release of step
-// s-1, earlier in its own program order, and the wgmma of step s+1, which warp 0 issued before it waited.  The same
-// holds across the pass change: the releases of the coarse pass's last two steps load the fine pass's first two
-// (the cursor runs on into the next pass), and those EMPTY waits are satisfied by the drains that end the coarse
-// pass's last MMA run, before the flush and its workers_sync.
+// tile), so steps alternate between slots 0-1 and 2-3.  A step's halves are released once the wgmma that read them
+// have completed (one step later: wait_group 1, or at the drain that ends an MMA run).  Each warp's lane 0 releases a
+// step with an acq_rel atomic add on the count of its slot pair, and the warp whose add completes the step's 4
+// releases (old count 3 mod 4) refills the pair at once with the step two ahead: nobody waits to refill.  Steps 0 and
+// 1 are loaded at kernel start.  A warpgroup never waits for the other one's refill, so the two may drift apart by up
+// to a step between two workers_sync, which staggers their use of the tensor pipe and of L2.
+//  * The count needs no reset: a warp releases step s + 2 (same slot pair) only after its FULL wait, whose load the
+//    last release of step s issued, so the 4 releases of one step are the 4 consecutive adds on their count.
+//  * Refills stay in slot order: a warp releases step s + 1 only after the refill it may have done at its release of s
+//    has returned, so the refill at the last release of s + 1 follows the refill of s.
+//  * Cursor visibility: the Feed writes of one refill happen before the refilling warp's release add of the next step
+//    on the other count, which the next refiller's add reads (acquire): the next refill sees the cursor advanced.
+//  * Pass change: the cursor runs on into the next pass's weight image, so the releases of the coarse pass's last two
+//    steps load the fine pass's first two, which arrive during the flush and the `ready` wait.
+// There is no wait on the refill path, so nothing to deadlock on; only acquire() waits, on FULL.
 // FAST (single-pass engine): the same sequence numbers and the same protocol on each step's first (W_hi) slot only;
 // the barriers of the W_lo slots are never used.
 template <bool FAST>
@@ -311,9 +328,12 @@ struct Ring {
   __device__ __forceinline__ void release(uint32_t s) {
     __syncwarp();
     if (lane == 0) {
-      mbar_arrive(bar_base + (BAR_EMPTY + s % NSLOTS) * 8);
-      if (!FAST) mbar_arrive(bar_base + (BAR_EMPTY + (s + 1) % NSLOTS) * 8);
-      if ((threadIdx.x & 127) == 0) feed_step<FAST>(bar_base, b_base, s + NSLOTS, threadIdx.x >> 7, status);
+      const int wg = threadIdx.x >> 7;
+      if (atom_add_acq_rel(smem_u32(&feed(wg).released[(s / 2) & 1]), 1) % 4 == 3) {
+        PROF_BEGIN(t0);
+        refill<FAST>(bar_base, b_base, s + NSLOTS, wg);
+        PROF_END_ANY(PH_REFILL, t0);
+      }
     }
     __syncwarp();
   }
@@ -674,32 +694,30 @@ __device__ __forceinline__ void field_tc(const Params& p) {
   PROF_INIT();
 
   if ((threadIdx.x & 127) == 0) {
-    for (int i = 0; i < NSLOTS; ++i) {
-      mbar_init(bar_base + (BAR_FULL + i) * 8, 1);
-      mbar_init(bar_base + (BAR_EMPTY + i) * 8, NCONSUMER_WARPS / 2);
-    }
+    for (int i = 0; i < NSLOTS; ++i) mbar_init(bar_base + (BAR_FULL + i) * 8, 1);
     if (threadIdx.x == 0) *n_list = 0;
     Feed& f = feed(wg);
     for (int i = 0; i < 2; ++i) {
-      f.slots[i] = i < p.npass ? p.pass[i].packed + HEADER_BYTES : nullptr;
+      f.slots[i] = i < p.npass ? p.pass[i].packed + HEADER_BYTES + wg * HALF_SLOT_BYTES : nullptr;
       f.n_tiles[i] = i < p.npass ? p.pass[i].n_tiles : 0;
     }
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(f.keep));
+    f.released[0] = f.released[1] = 0;
     f.npass = p.npass;
     f.NS = NS;
     f.pair = pair;
     f.n_pairs = n_pairs;
     f.ps = 0;
     f.v = 0;
-    f.i = 0;
     f.tile = pair;
-    f.skip_empty_passes();
+    f.begin_run();
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   if ((threadIdx.x & 127) == 0) {
-    // prefill: steps 0 and 1 (the EMPTY waits of the first use of a slot return at once)
-    feed_step<FAST>(bar_base, b_base, 0, wg, p.status);
-    feed_step<FAST>(bar_base, b_base, 2, wg, p.status);
+    // prefill: steps 0 and 1
+    refill<FAST>(bar_base, b_base, 0, wg);
+    refill<FAST>(bar_base, b_base, 2, wg);
   }
   const size_t map_stride = (size_t)p.sc.SB * NS * p.sc.Hl * p.sc.Wl * D;
 

@@ -293,20 +293,30 @@ __device__ __forceinline__ void refill(uint32_t bar_base, uint32_t b_base, uint3
 // with its own FULL mbarriers, release counts and Feed cursor; the two rings share nothing.  The halves are filled in
 // exactly the order the warpgroup uses them; every step takes two consecutive slots (W_hi, W_lo of one 128-row x 64-k
 // tile), so steps alternate between slots 0-1 and 2-3.  A step's halves are released once the wgmma that read them
-// have completed (one step later: wait_group 1, or at the drain that ends an MMA run).  Each warp's lane 0 releases a
-// step with an acq_rel atomic add on the count of its slot pair, and the warp whose add completes the step's 4
-// releases (old count 3 mod 4) refills the pair at once with the step two ahead: nobody waits to refill.  Steps 0 and
-// 1 are loaded at kernel start.  A warpgroup never waits for the other one's refill, so the two may drift apart by up
-// to a step between two workers_sync, which staggers their use of the tensor pipe and of L2.
-//  * The count needs no reset: a warp releases step s + 2 (same slot pair) only after its FULL wait, whose load the
-//    last release of step s issued, so the 4 releases of one step are the 4 consecutive adds on their count.
-//  * Refills stay in slot order: a warp releases step s + 1 only after the refill it may have done at its release of s
-//    has returned, so the refill at the last release of s + 1 follows the refill of s.
+// have completed: at the next step's acquire(), which retires the step (wait_group 0) and releases it BEFORE it waits
+// for the next step's slots, or at the drain that ends an MMA run.  Each warp's lane 0 releases a step with an
+// acq_rel atomic add on the count of its slot pair, and the warp whose add completes the step's 4 releases (old count
+// 3 mod 4) refills the pair at once with the step two ahead: nobody waits to refill.  So while a warpgroup waits for
+// step s + 1 to land, the copy of step s + 2 is already in flight beside it; releasing s only after s + 1 had landed
+// and been issued (wait_group 1 after the commit of s + 1) left one copy in flight per warpgroup, and the step period
+// was a whole L2 -> shared-memory round trip.  Steps 0 and 1 are loaded at kernel start.  A warpgroup never waits for
+// the other one's refill, so the two may drift apart by up to a step between two workers_sync, which staggers their
+// use of the tensor pipe and of L2; while one warpgroup waits for its step to retire, the other's wgmma keep the
+// tensor pipe busy.
+//  * The count needs no reset: a warp releases step s + 2 (same slot pair) only after its FULL wait for s + 2, whose
+//    load the last release of step s issued, so the 4 releases of one step are the 4 consecutive adds on their count.
+//  * No slot is freed under a reader: the release follows wait_group 0, when every wgmma of the warp's warpgroup that
+//    read the step has completed.  Every warp runs the same wait_group sequence (none depends on data).
+//  * Refills stay in slot order: each warp releases every step once and in step order, and releases step s + 1 only
+//    after the refill it may have done at its release of s has returned, so the refill at the last release of s + 1
+//    follows the refill of s.
 //  * Cursor visibility: the Feed writes of one refill happen before the refilling warp's release add of the next step
 //    on the other count, which the next refiller's add reads (acquire): the next refill sees the cursor advanced.
 //  * Pass change: the cursor runs on into the next pass's weight image, so the releases of the coarse pass's last two
-//    steps load the fine pass's first two, which arrive during the flush and the `ready` wait.
-// There is no wait on the refill path, so nothing to deadlock on; only acquire() waits, on FULL.
+//    steps (at the drains that end the pass) load the fine pass's first two, which arrive during the flush and the
+//    `ready` wait.
+// There is no wait on the refill path, so nothing to deadlock on; only acquire() waits, on FULL, after its own warp
+// has released every earlier step (the other warps release theirs without waiting for anything).
 // FAST (single-pass engine): the same sequence numbers and the same protocol on each step's first (W_hi) slot only;
 // the barriers of the W_lo slots are never used.
 template <bool FAST>
@@ -318,7 +328,15 @@ struct Ring {
   int lane;
   int* status;
   __device__ __forceinline__ uint32_t slot_addr(uint32_t s) const { return b_base + (s % NSLOTS) * SLOT_BYTES; }
+  // retire and release the step before (its refill leaves now), then wait for this step's slots
   __device__ __forceinline__ void acquire() {
+    if (has_pend) {
+      PROF_BEGIN(t1);
+      wgmma_wait<0>();
+      PROF_END(PH_WGMMA_WAIT, t1);
+      release(pend);
+      has_pend = false;
+    }
     PROF_BEGIN(t0);
     for (uint32_t s = seq; s < seq + (FAST ? 1 : 2); ++s)
       mbar_wait(bar_base + (BAR_FULL + s % NSLOTS) * 8, (s / NSLOTS) & 1, status,
@@ -337,13 +355,9 @@ struct Ring {
     }
     __syncwarp();
   }
-  // after the step's wgmma are issued: commit them as one group, retire the previous step
+  // after the step's wgmma are issued: commit them as one group (the next acquire() or drain() retires it)
   __device__ __forceinline__ void issued() {
     wgmma_commit();
-    PROF_BEGIN(t0);
-    wgmma_wait<1>();
-    PROF_END(PH_WGMMA_WAIT, t0);
-    if (has_pend) release(pend);
     pend = seq;
     has_pend = true;
     seq += 2;

@@ -38,18 +38,18 @@ def build_net(case, device="cuda:0", engine="auto"):
     return net
 
 
-def build_renderer(case):
+def build_renderer(case, depth_std=0.01):
     from render import NeRFRenderer
     cfg = case["cfg"]
     r = NeRFRenderer(n_coarse=cfg["n_coarse"], n_fine=cfg["n_fine"], n_fine_depth=cfg["n_fine_depth"],
-                     depth_std=0.01, white_bkgd=bool(cfg["white_bkgd"]), eval_batch_size=cfg["eval_batch_size"])
+                     depth_std=depth_std, white_bkgd=bool(cfg["white_bkgd"]), eval_batch_size=cfg["eval_batch_size"])
     return r.eval()
 
 
-def render_case_cuda(case, engine="auto", device="cuda:0"):
+def render_case_cuda(case, engine="auto", device="cuda:0", depth_std=0.01):
     """Fused render of a golden case with the fixture's noise -> dict like oracle.render."""
     net = build_net(case, device, engine)
-    renderer = build_renderer(case)
+    renderer = build_renderer(case, depth_std)
     rays = case["rays"].to(device)
     noise = {k: v.to(device) for k, v in case["noise"].items()}
     with torch.no_grad():

@@ -9,7 +9,7 @@ import torch
 
 import emu_util as eu
 import golden_util as gu
-from test_emu_kernels import _emulated_training_step, rel
+from test_emu_kernels import _emulated_training_step, fine_checked, rel
 
 bw = gu.load_by_path("pnr_backward", os.path.join(gu.ROOT, "oracle", "pnr_backward.py"))
 synth, oracle = gu.synth, gu.oracle
@@ -64,15 +64,12 @@ def test_random_configuration(seed):
     assert (t["z_coarse"] - ref["coarse"]["z"]).abs().max() < 1e-6
     assert (t["rgb_coarse"] - ref["coarse"]["rgb"]).abs().max() < 1e-4
     assert (t["weights_coarse"] - ref["coarse"]["weights"]).abs().max() < 1e-4
-    same_samples = True
     if cfg["n_fine"] > 0:
-        flipped = ((t["z_fine"] - ref["fine"]["z"]).abs() > 2e-4).any(-1)
-        assert int(flipped.sum()) <= 1
-        same_samples = not bool(flipped.any())
-        assert (t["rgb_fine"] - ref["fine"]["rgb"])[~flipped].abs().max() < 1e-4
-        assert torch.all(t["z_fine"][:, 1:] >= t["z_fine"][:, :-1])
-    if not same_samples:
-        pytest.skip("an importance sample flipped a CDF bin: gradients are not comparable for this seed")
+        fine_checked(case, t)
+        if ((t["z_fine"] - ref["fine"]["z"]).abs() > 2e-4).any():
+            # the forward was checked above on the emulator's own samples; the oracle backward below replays the
+            # oracle's samples, so its gradients are comparable only where both took the same bins
+            pytest.skip("an importance sample took a bin next to the oracle's: gradients are not comparable")
     m_loss, o_c, o_f, o_lat = bw.train_loss_backward(case["rays"], gt, case["noise"], gu.oracle_state(case),
                                                      case["latent"], case["wc"], case["wf"], cfg["NS"],
                                                      cfg["n_coarse"], cfg["n_fine"], cfg["n_fine_depth"],

@@ -1,10 +1,12 @@
 """GPU parity: the CUDA path (through the Python surface and the C ABI) against the CPU
 oracle on the golden cases.  Tolerances: |d rgb| < 1e-4 (BASELINE.json north_star),
-sample depths / weights 1e-5; fine-pass comparisons exclude rays whose importance samples
-flipped a CDF bin (a 1-ulp effect of searchsorted, counted and bounded)."""
+sample depths / weights 1e-5.  The fine pass is checked on every ray against a reference conditioned on the
+kernel's own coarse pass (tests/fine_pass_check.py): an importance sample may take the bin next to the oracle's only
+when its u lies within fp32 rounding of the cdf edge between them."""
 import pytest
 import torch
 
+import fine_pass_check as fpc
 import golden_util as gu
 
 pytestmark = pytest.mark.gpu
@@ -13,10 +15,6 @@ pytestmark = pytest.mark.gpu
 # default: engine "auto" picks it whenever the shape allows)
 TC_CASES = ["c2_small", "c3_small", "c4_small"]
 CASE_ENGINE = [(n, "simt") for n in gu.CASE_NAMES] + [(n, "tc") for n in TC_CASES] + [(n, "auto") for n in TC_CASES]
-
-
-def _flipped_rays(z_a, z_b, tol=2e-4):
-    return ((z_a - z_b).abs() > tol).any(dim=-1)
 
 
 @pytest.mark.parametrize("name,engine", CASE_ENGINE)
@@ -31,13 +29,9 @@ def test_render_parity(name, engine):
     assert (c["depth"].cpu() - rc["depth"]).abs().max() < 1e-4
     assert (c["weights"].cpu() - rc["weights"]).abs().max() < 1e-4
     if case["cfg"]["n_fine"] > 0:
-        f, rf = res["fine"], ref["fine"]
-        flipped = _flipped_rays(f["z"].cpu(), rf["z"])
-        assert flipped.float().mean() <= 0.05, f"{int(flipped.sum())} rays flipped a CDF bin"
-        ok = ~flipped
-        assert (f["rgb"].cpu()[ok] - rf["rgb"][ok]).abs().max() < 1e-4
-        assert (f["depth"].cpu()[ok] - rf["depth"][ok]).abs().max() < 1e-4
-        assert torch.all(f["z"][:, 1:] >= f["z"][:, :-1])  # sorted
+        chk = fpc.check_case(case, res)
+        flipped = int(((res["fine"]["z"].cpu() - ref["fine"]["z"]).abs() > 2e-4).any(-1).sum())
+        print(f"{name} {engine}: {chk}, {flipped} rays merged other samples than the oracle")
 
 
 @pytest.mark.parametrize("name,engine", CASE_ENGINE)
@@ -91,9 +85,9 @@ def test_stage_entry_points():
     pn.check(L.pnr_sample_fine(pn.dptr(rays), pn.dptr(zc_ref), pn.dptr(wc_ref), pn.dptr(dc_ref), pn.dptr(u_f), pn.dptr(u_j),
                                pn.dptr(n_d), 0.01, pn.dptr(zf), R, Kc, Kf, Kfd, sp))
     torch.cuda.synchronize()
-    flipped = _flipped_rays(zf.cpu(), ref["fine"]["z"])
-    assert flipped.float().mean() <= 0.03
-    assert (zf.cpu()[~flipped] - ref["fine"]["z"][~flipped]).abs().max() < 1e-5
+    # the oracle's coarse pass as input: every ray's merge explained against the float64 cdf of those weights
+    moved = fpc.explain_fine_z(rays, zc_ref, wc_ref, dc_ref, n, Kc, Kf, Kfd, 0.01, zf)
+    print(f"pnr_sample_fine on the oracle's coarse pass: {moved} importance samples in a non-float64 bin")
 
 
 @pytest.mark.parametrize("name,engine", [("tiny", "simt"), ("c2_small", "auto")])
@@ -139,8 +133,7 @@ def test_sample_count_edge_cases(n_fine, n_fine_depth, name, engine):
     ref = gu.oracle_render(case)
     assert (res["coarse"]["rgb"].cpu() - ref["coarse"]["rgb"]).abs().max() < 1e-4
     if n_fine > 0:
-        flipped = ((res["fine"]["z"].cpu() - ref["fine"]["z"]).abs() > 2e-4).any(dim=-1)
-        assert flipped.float().mean() <= 0.1
-        assert (res["fine"]["rgb"].cpu()[~flipped] - ref["fine"]["rgb"][~flipped]).abs().max() < 1e-4
+        chk = fpc.check_case(case, res, depth_tol=2e-4)
+        print(f"{name} {engine} ({n_fine}, {n_fine_depth}): {chk}")
     else:
         assert "fine" not in res

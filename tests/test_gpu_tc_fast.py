@@ -1,8 +1,8 @@
 """The single-pass tensor engine (engine "tc_fast", PNR_ENGINE_TC_FAST) on the H100: against its CPU restatement
 (tests/tc_fast_oracle.py) at a tight bound, against the fp32 oracle at the documented loose bound, at the true C2 / C3 /
 C4 shapes, through bind_parallel and util.recon, and its refusals (grad mode, the backward entry points, shapes the
-tensor engine cannot run).  Fine-pass comparisons exclude rays whose importance samples flipped a CDF bin, as
-tests/test_gpu_parity.py does; the flips are counted and bounded."""
+tensor engine cannot run).  The fine pass is checked on every ray against references conditioned on the kernel's own
+coarse pass (tests/fine_pass_check.py)."""
 import ctypes as C
 import importlib.util
 import os
@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+import fine_pass_check as fpc
 import golden_util as gu
 import gpu_util
 import tc_fast_oracle as fo
@@ -27,7 +28,6 @@ PNR_ERR_INVALID = -1              # include/pnr.h
 PARITY_MAX_DRGB = 2e-3
 PARITY_P999_DRGB = 2e-3
 PARITY_PSNR_DB = 55.0
-PARITY_FLIPPED = 160              # of 256 rays: C4's fine samples flip a bin on 44 % of them
 RECON_SIGMA = 5e-3                # util.recon sigma grid: max |d sigma| / (1 + max |sigma|); measured 5.2e-4
 
 
@@ -46,11 +46,13 @@ def test_render_against_restatement_and_oracle(name):
     loose = fo.render_errors(res, ref)
     print(f"{name}: vs restatement {tight}  vs fp32 oracle {loose}")
     assert (res["coarse"]["z"] - ref["coarse"]["z"]).abs().max() < 1e-6      # the stratified samples are exact
-    assert tight["coarse"] < fo.TIGHT_RGB and tight["fine"] < fo.TIGHT_RGB, tight
-    assert tight["flipped"] <= tight["rays"] // 2, tight        # measured: 0, 0 and 6 of 16 rays
-    assert loose["coarse"] < fo.LOOSE_RGB and loose["fine"] < fo.LOOSE_RGB, loose
-    assert loose["flipped"] <= tight["rays"] // 2, loose        # measured: 0, 1 and 5 of 16 rays
-    assert torch.all(res["fine"]["z"][:, 1:] >= res["fine"]["z"][:, :-1])
+    assert tight["coarse"] < fo.TIGHT_RGB, tight
+    assert loose["coarse"] < fo.LOOSE_RGB, loose
+    # every ray's fine pass at the kernel's own samples: against the restatement and against the fp32 oracle
+    chk = fpc.check_case(case, res, arithmetic=fo.arithmetic, rgb_tol=fo.TIGHT_RGB, depth_tol=None, weights_tol=None)
+    chk_loose = fpc.check_fine_outputs(case["rays"], res["fine"]["z"], res["fine"], fpc.case_composite(case),
+                                       rgb_tol=fo.LOOSE_RGB, depth_tol=None, weights_tol=None)
+    print(f"{name} tc_fast: vs restatement {chk}  vs fp32 oracle {chk_loose}")
 
 
 @pytest.mark.parametrize("name", CASES)
@@ -118,7 +120,11 @@ def test_parity_block_at_true_shapes(name):
     assert par["max_abs_drgb"] < PARITY_MAX_DRGB, par
     assert par["p999_abs_drgb"] < PARITY_P999_DRGB, par
     assert par["psnr_db"] > PARITY_PSNR_DB, par
-    assert par["flipped_rays"] <= PARITY_FLIPPED, par
+    # the same rays and noise, every ray's fine pass checked; the float64 restatement on a fixed subset of them
+    chk = fpc.check_true_shape(bench, net, renderer, cfg, rays, n=256, arithmetic=fo.arithmetic, n_sub=96,
+                               rgb_tol=fo.TIGHT_RGB, depth_tol=None, weights_tol=None)
+    assert pn.tc_status() == 0
+    print(f"{name} tc_fast: vs restatement {chk}")
 
 
 def test_bind_parallel_two_shards_bit_equal_to_one_gpu():

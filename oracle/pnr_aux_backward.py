@@ -45,9 +45,7 @@ def composite_backward(rays, z, field, d_rgb, d_depth, d_weights, white_bkgd):
         g_w = g_w - d_rgb.sum(-1, keepdim=True)
     if d_weights is not None:
         g_w = g_w + d_weights
-    gw_w = g_w * w
-    suffix = torch.flip(torch.cumsum(torch.flip(gw_w, [1]), 1), [1]) - gw_w     # sum_{m>k} g_w,m w_m
-    d_a = g_w * T - suffix / t
+    d_a = g_w * T - bw.exclusive_suffix(g_w * w) / t
     d_s = d_a * e * deltas
     d_delta = d_a * e * s
     d_field = torch.empty_like(field)

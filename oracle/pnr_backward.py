@@ -43,6 +43,13 @@ def _linear(x, w, b):
 # ----------------------------------------------------------------------------------------
 # compositing (nerf.py:178-182, 222-249)
 # ----------------------------------------------------------------------------------------
+def exclusive_suffix(x):
+    """sum_{m>k} x_m along the last axis, summed from the back.  Not (inclusive sum - x_k): behind a near-opaque sample
+    both terms are that sample's g w and their difference, later divided by t_k ~ 1e-4 .. 1e-10, is all rounding."""
+    rev = torch.flip(torch.cumsum(torch.flip(x, [-1]), -1), [-1])
+    return torch.cat([rev[..., 1:], torch.zeros_like(rev[..., :1])], -1)
+
+
 def composite_backward(rays, z, field, d_rgb, d_depth, white_bkgd):
     """field (B,K,4) = (rgb_k, sigma_k) as PixelNeRFNet.forward returns them; d_rgb (B,3), d_depth (B,).
     Forward: delta_k = z_{k+1} - z_k (last: far - z_{K-1}); s_k = relu(sigma_k); e_k = exp(-delta_k s_k);
@@ -61,9 +68,7 @@ def composite_backward(rays, z, field, d_rgb, d_depth, white_bkgd):
     g_w = (d_rgb.unsqueeze(1) * c).sum(-1) + d_depth.unsqueeze(1) * z
     if white_bkgd:
         g_w = g_w - d_rgb.sum(-1, keepdim=True)
-    gw_w = g_w * w
-    suffix = torch.flip(torch.cumsum(torch.flip(gw_w, [1]), 1), [1]) - gw_w     # sum_{m>k} g_w,m w_m
-    d_a = g_w * T - suffix / t
+    d_a = g_w * T - exclusive_suffix(g_w * w) / t
     d_s = d_a * e * deltas
     d_delta = d_a * e * s
     d_field = torch.empty_like(field)

@@ -243,8 +243,12 @@ int launch_frames_u8(const float* rgb, int64_t n, uint8_t* out, cudaStream_t s) 
 
 // ----------------------------------------------------------------------------------------
 // Backward of the renderer's own arithmetic (oracle/pnr_aux_backward.py::composite_backward / render_backward, which
-// extend oracle/pnr_backward.py's rgb-only formulas).  One thread per ray; two sweeps over the K samples instead of
-// storing per-sample state: sweep 1 accumulates S = sum_k g_k w_k, sweep 2 turns the running prefix into the transmittance suffix sums.
+// extend oracle/pnr_backward.py's rgb-only formulas).  One thread per ray; two sweeps over the K samples and no
+// per-sample state beyond the outputs.  With t_k = (1 - a_k) + 1e-10 and T_k = prod_{j<k} t_j, the alpha gradient is
+//   d_a_k = g_k T_k - sum_{m>k} g_m w_m / t_k = T_k (g_k - U_k),   U_k = sum_{m>k} g_m a_m prod_{k<j<m} t_j,
+// and U follows U_{K-1} = 0, U_{k-1} = g_k a_k + t_k U_k.  Sweep 1 runs back to front and parks U_k in d_z[k] (which
+// sweep 2 overwrites); sweep 2 runs front to back with T.  No suffix is formed as a difference and nothing is divided
+// by t: behind a near-opaque sample t is 1e-4 .. 1e-10, and (total - prefix) / t there loses every bit to cancellation.
 // The per-sample weight gradient is g_k = d_rgb . c_k + d_depth z_k (- sum d_rgb on a white background) + d_weights_k;
 // any of the three upstream gradients may be NULL (zero).  Without d_weights the arithmetic is that of the rgb/depth-only
 // kernel bit for bit (the add is skipped, not done with 0).
@@ -258,27 +262,27 @@ __global__ void k_composite_bwd(const float* __restrict__ rays, const float* __r
   if (r >= R) return;
   const float far = rays[r * 8 + 7];
   const float* zr = z + r * K;
+  float* dzr = d_z + r * K;
   const float4* fr = reinterpret_cast<const float4*>(field) + r * K;
   const float* dwr = d_weights ? d_weights + r * K : nullptr;
   const float gr = d_rgb ? d_rgb[r * 3 + 0] : 0.f, gg = d_rgb ? d_rgb[r * 3 + 1] : 0.f,
               gb = d_rgb ? d_rgb[r * 3 + 2] : 0.f;
   const float gd = d_depth ? d_depth[r] : 0.f;
   const float gbg = white ? (gr + gg + gb) : 0.f;   // rgb += 1 - sum w  (nerf.py:241-244)
-  float S = 0.f;
   {
-    float T = 1.0f, zk = zr[0];
-    for (int k = 0; k < K; ++k) {
-      const float znext = (k + 1 < K) ? zr[k + 1] : far;
+    float U = 0.f, znext = far;
+    for (int k = K - 1; k >= 0; --k) {
+      dzr[k] = U;
+      const float zk = zr[k];
       const float4 f = fr[k];
-      const float alpha = 1.0f - expf(-(znext - zk) * fmaxf(f.w, 0.f));
+      const float alpha = 1.0f - expf(-(znext - zk) * fmaxf(f.w, 0.f));    // sweep 2's e and alpha, same roundings
       float gw = ((gr * f.x + gg * f.y) + gb * f.z) + gd * zk - gbg;
       if (dwr) gw += dwr[k];
-      S += gw * (alpha * T);
-      T = T * ((1.0f - alpha) + 1e-10f);
-      zk = znext;
+      U = gw * alpha + ((1.0f - alpha) + 1e-10f) * U;
+      znext = zk;
     }
   }
-  float T = 1.0f, zk = zr[0], prefix = 0.f, carry = 0.f;
+  float T = 1.0f, zk = zr[0], carry = 0.f;
   float4* dfr = reinterpret_cast<float4*>(d_field) + r * K;
   for (int k = 0; k < K; ++k) {
     const float znext = (k + 1 < K) ? zr[k + 1] : far;
@@ -291,14 +295,13 @@ __global__ void k_composite_bwd(const float* __restrict__ rays, const float* __r
     const float w = alpha * T;
     float gw = ((gr * f.x + gg * f.y) + gb * f.z) + gd * zk - gbg;
     if (dwr) gw += dwr[k];
-    prefix += gw * w;
-    const float d_a = gw * T - (S - prefix) / t;      // S - prefix = sum_{m>k} g_m w_m
+    const float d_a = T * (gw - dzr[k]);              // dzr[k] = U_k from sweep 1
     const float d_delta = d_a * e * sg;
     float4 o;
     o.x = w * gr; o.y = w * gg; o.z = w * gb;
     o.w = (f.w > 0.f) ? d_a * e * delta : 0.f;
     dfr[k] = o;
-    d_z[r * K + k] = (w * gd - d_delta) + carry;       // delta_{k-1} = z_k - z_{k-1} gives +d_delta_{k-1}
+    dzr[k] = (w * gd - d_delta) + carry;               // delta_{k-1} = z_k - z_{k-1} gives +d_delta_{k-1}
     carry = d_delta;
     T = T * t;
     zk = znext;

@@ -20,12 +20,13 @@
 //  * lin_z[i](latent) is NOT a per-sample GEMM: bilinear interpolation commutes with a linear
 //    layer, so pnr_project_latent builds P_i = lin_z[i](latent) (+ biases) once per encode()
 //    and the epilogue gathers 4 taps of P_i and adds them to the residual stream.
-//  * 256 threads = two warpgroups (geometry, wgmma, epilogues, ray finishing), so ptxas may give each thread 255
-//    registers: the 160 accumulator registers plus addressing fit, and each step's 9 or 12 wgmma issue back to back
-//    as one commit group.  There is no weight-stream warp: each warpgroup has its own 4-slot ring of the 8 KB halves
-//    of the pre-swizzled 16 KB weight tiles that it multiplies, which the last of its warps to release a step's slots
-//    refills at once (cp.async.bulk in consumption order onto FULL mbarriers; struct Ring).
-//    tests/test_tc_codegen.py guards the register budget.
+//  * 384 threads = two consumer warpgroups (geometry, wgmma, epilogues, ray finishing) and one producer warpgroup.
+//    setmaxnreg moves the producer down to 40 registers per thread and the consumers up to 232: the 160 accumulator
+//    registers plus addressing fit, and each step's 9 or 12 wgmma issue back to back as one commit group.  Each
+//    consumer warpgroup has its own 4-slot ring of the 8 KB halves of the pre-swizzled 16 KB weight tiles that it
+//    multiplies; its warps only release a step's slots, and one lane of the producer warpgroup per ring refills them
+//    (cp.async.bulk in consumption order onto FULL mbarriers; struct Ring, produce()), so the warps that issue wgmma
+//    never stop to refill.  tests/test_tc_codegen.py and tests/test_tc_producer.py guard the register budget.
 //  * k_field_tc_fast (PNR_ENGINE_TC_FAST) is the same body with FAST = true: one tensor pass per step, D += Ahi*Whi
 //    with fp32 accumulation.  It loads only the W_hi tile of each step (the W_lo slot of the ring stays idle) and never
 //    writes the fp16 lo halves of its A operands.  The projected-latent gather (lin_z stays exact), geometry, the view
@@ -52,7 +53,13 @@ constexpr int ROWS = 64;                 // rows (points) per CTA
 constexpr int TILE_POINTS = 128;         // per tile index (two CTAs)
 constexpr int NCONSUMER_WARPS = 8;       // two warpgroups
 constexpr int NCONSUMERS = NCONSUMER_WARPS * 32;
-constexpr int NTHREADS = NCONSUMERS;     // thread 0 also issues the weight-slot loads (no dedicated streamer warp)
+constexpr int NTHREADS = NCONSUMERS + 128;   // + the producer warpgroup, which issues the weight-slot loads
+// setmaxnreg budgets: the launch gives every thread 65536 / 384 -> 168 registers; the producer returns what the
+// consumers take
+constexpr int PRODUCER_REGS = 40;
+constexpr int CONSUMER_REGS = 232;
+static_assert(128 * PRODUCER_REGS + NCONSUMERS * CONSUMER_REGS <= NTHREADS * 168,
+              "the consumers take no more registers than the producer returns");
 constexpr int SLOT_BYTES = 16384;        // 128 weight rows x 64 k x fp16
 constexpr int HALF_SLOT_BYTES = SLOT_BYTES / 2;   // rows [64g, 64g+64) of a slot: the half warpgroup g reads
 constexpr int NSLOTS = 4;
@@ -72,13 +79,13 @@ constexpr int SM_AH = SM_A + A_BYTES;                   // 131072
 constexpr int SM_B = SM_AH + AH_BYTES;                  // 163840
 constexpr int SM_GEO = SM_B + NSLOTS * SLOT_BYTES;      // [64][8] words: 4 tap offsets + 4 bilinear weights per row
 constexpr int SM_PART = SM_A;                           // lin_out partials [64][2][4] floats alias A chunk 0 (free at tile end)
-constexpr int SM_BAR = SM_GEO + ROWS * 8 * 4;          // [2][BAR_COUNT]: the mbarriers of each warpgroup's ring
-constexpr int BAR_FULL = 0;                             // [NSLOTS]
+constexpr int SM_BAR = SM_GEO + ROWS * 8 * 4;          // [2][RING_BYTES]: each warpgroup's ring control
+constexpr int BAR_FULL = 0;                             // [NSLOTS] mbarriers
 constexpr int BAR_COUNT = BAR_FULL + NSLOTS;
-constexpr int SM_NLIST = SM_BAR + 2 * BAR_COUNT * 8;    // fused render: number of rays this CTA completed in the current pass
-constexpr int SM_FEED = SM_NLIST + 16;                  // struct Feed [2]: the refill cursor and release counts of each ring
-constexpr int FEED_BYTES = 128;
-constexpr int SM_PROF = SM_FEED + 2 * FEED_BYTES;       // phase counters of the profile build: [2][PH_COUNT] u64
+constexpr int RING_RELEASED = BAR_COUNT * 8;            // [2] u32: the release counts of the ring's two slot pairs
+constexpr int RING_BYTES = RING_RELEASED + 8;
+constexpr int SM_NLIST = SM_BAR + 2 * RING_BYTES;       // fused render: number of rays this CTA completed in the current pass
+constexpr int SM_PROF = SM_NLIST + 16;                  // phase counters of the profile build: [2][PH_COUNT] u64
 #ifdef PNR_TC_PROFILE
 constexpr int SMEM_BYTES = SM_PROF + 128;
 #else
@@ -135,18 +142,18 @@ using namespace tcptx;
 enum { MODE_GATHER = 0, MODE_BIAS_WB = 1, MODE_COMBINE = 2, MODE_OUT = 3 };
 
 // Phase profile (built with -DPNR_TC_PROFILE into lib/libpnr_sm90_prof.so, scripts/tc_phase_profile.py): the first
-// thread of each warpgroup adds the clock64() time it spends in each phase to a shared-memory counter and, at kernel
-// end, to the 8 counters that pnr_tc_counters returns.  The exception is PH_REFILL: the time spent issuing the ring's
-// refills, counted on whichever lane 0 releases a step last and so refills (struct Ring); a ring's refills never
-// overlap, so that plain add does not race.  The phases of the first thread are disjoint; the rest of PH_TOTAL is
-// wgmma issue and the epilogue arithmetic.  The hooks are macros that the production build expands to nothing, so its
-// kernels are the same instructions with or without them (tests/test_tc_profile.py).
+// thread of each consumer warpgroup adds the clock64() time it spends in each phase to a shared-memory counter and, at
+// kernel end, to the 8 counters that pnr_tc_counters returns.  The exception is PH_REFILL: the time each ring's
+// producer lane spends issuing its refills (not waiting for releases), which it adds to the global counter itself when
+// its ring is done (produce()).  The phases of the first thread are disjoint; the rest of PH_TOTAL is wgmma issue and
+// the epilogue arithmetic.  The hooks are macros that the production build expands to nothing, so its kernels are the
+// same instructions with or without them (tests/test_tc_profile.py).
 #ifdef PNR_TC_PROFILE
 extern __shared__ __align__(1024) uint8_t smem[];
 enum { PH_FULL, PH_REFILL, PH_WGMMA_WAIT, PH_SYNC, PH_GATHER, PH_GEOM, PH_FLUSH, PH_TOTAL, PH_COUNT };
-__device__ __forceinline__ void prof_add(int ph, long long t0, bool any_thread = false) {
+__device__ __forceinline__ void prof_add(int ph, long long t0) {
   const long long dt = clock64() - t0;
-  if (any_thread || (threadIdx.x & 127) == 0)
+  if ((threadIdx.x & 127) == 0)
     reinterpret_cast<unsigned long long*>(smem + SM_PROF)[(threadIdx.x >> 7) * PH_COUNT + ph] += (unsigned long long)dt;
 }
 __device__ __forceinline__ void prof_finish(int* status, long long t_kernel) {
@@ -159,18 +166,23 @@ __device__ __forceinline__ void prof_finish(int* status, long long t_kernel) {
 #define PROF_BEGIN(t) long long t = clock64()
 #define PROF_RESTART(t) t = clock64()
 #define PROF_END(ph, t) prof_add(ph, t)
-#define PROF_END_ANY(ph, t) prof_add(ph, t, true)
 // before the kernel's first __syncthreads
 #define PROF_INIT() \
   if (threadIdx.x < 2 * PH_COUNT) reinterpret_cast<unsigned long long*>(smem + SM_PROF)[threadIdx.x] = 0
 #define PROF_FINISH(status, t) prof_finish(status, t)
+// a producer lane's private sum of one phase, added to the global counter when the lane is done
+#define PROF_SUM_INIT(s) long long s = 0
+#define PROF_SUM(s, t) s += clock64() - (t)
+#define PROF_PUBLISH(status, ph, s) atomicAdd(reinterpret_cast<unsigned long long*>((status) + 2) + (ph), (unsigned long long)(s))
 #else
 #define PROF_BEGIN(t)
 #define PROF_RESTART(t)
 #define PROF_END(ph, t)
-#define PROF_END_ANY(ph, t)
 #define PROF_INIT()
 #define PROF_FINISH(status, t)
+#define PROF_SUM_INIT(s)
+#define PROF_SUM(s, t)
+#define PROF_PUBLISH(status, ph, s)
 #endif
 
 __device__ __forceinline__ void workers_sync() {
@@ -220,41 +232,38 @@ extern __shared__ __align__(1024) uint8_t smem[];
 
 // The weight-slot sequence of one CTA, in consumption order: per pass, per tile of its pair, NS x (lin_in + blocks
 // 0-2: slots [0, SLOTS_HEAD) of the pass's weight image) then blocks 3-4 (slots [SLOTS_HEAD, SLOTS_TOTAL)), i.e. runs
-// of consecutive slots.  Each ring walks it one step (two slots: W_hi, W_lo of one tile) per refill.  The cursor lives
-// in shared memory so that no register is held for it across the MMA loops, and it keeps the next step's source
-// address and the steps left in its run, so that a refill inside a run reads two words and writes them back; only the
-// refill that ends a run walks on to the next view, tile or pass.
+// of consecutive slots.  The producer lane of ring g walks it one step (two slots: W_hi, W_lo of one tile) at a time
+// in registers; only the step that ends a run reads the kernel parameters to walk on to the next view, tile or pass.
 struct Feed {
-  const uint8_t* src;        // this warpgroup's half of the next step's W_hi slot; nullptr: the sequence is done
-  uint64_t keep;             // createpolicy evict_last for the weight images
-  int left;                  // steps left in the current run
-  uint32_t released[2];      // warp releases of the steps that use ring slots 0-1 / 2-3 (never reset: see Ring)
-  const uint8_t* slots[2];   // this warpgroup's half of the first slot of each pass's weight image
-  int64_t n_tiles[2];
+  const uint8_t* src;        // ring g's half of the next step's W_hi slot; nullptr: the sequence is done
   int64_t tile;              // tile of the current run
-  int npass, NS, pair, n_pairs;
+  int left;                  // steps left in the current run
   int ps, v;                 // pass (npass: sequence done), view of the current run (NS: the blocks 3-4 run)
-  __device__ __forceinline__ void begin_run() {
-    while (ps < npass && tile >= n_tiles[ps]) {
+  __device__ __forceinline__ void begin_run(const Params& p, int g) {
+    while (ps < p.npass && tile >= p.pass[ps].n_tiles) {
       ++ps;
-      tile = pair;
+      tile = blockIdx.x >> 1;
     }
-    const bool head = v < NS;
-    src = ps < npass ? slots[ps] + (head ? 0 : (size_t)SLOTS_HEAD * SLOT_BYTES) : nullptr;
+    const bool head = v < p.sc.NS;
+    src = ps < p.npass ? p.pass[ps].packed + HEADER_BYTES + g * HALF_SLOT_BYTES +
+                             (head ? 0 : (size_t)SLOTS_HEAD * SLOT_BYTES)
+                       : nullptr;
     left = (head ? SLOTS_HEAD : SLOTS_TAIL) / 2;
   }
-  __device__ __forceinline__ void next_run() {
-    if (++v > NS) {
-      v = 0;
-      tile += n_pairs;
+  __device__ __forceinline__ void next(const Params& p, int g) {
+    if (--left > 0) {
+      src += 2 * SLOT_BYTES;
+      return;
     }
-    begin_run();
+    if (++v > p.sc.NS) {
+      v = 0;
+      tile += gridDim.x >> 1;
+    }
+    begin_run(p, g);
   }
 };
-static_assert(sizeof(Feed) <= FEED_BYTES, "Feed does not fit its shared-memory slot");
 static_assert(SLOTS_HEAD % 2 == 0 && SLOTS_TAIL % 2 == 0, "a step's two slots lie in one run");
-static_assert(SM_PROF <= SMEM_BYTES, "the two rings' barriers and cursors fit under the block limit");
-__device__ __forceinline__ Feed& feed(int wg) { return *reinterpret_cast<Feed*>(smem + SM_FEED + wg * FEED_BYTES); }
+static_assert(SM_PROF <= SMEM_BYTES, "the two rings' barriers and release counts fit under the block limit");
 
 __device__ __forceinline__ uint32_t atom_add_acq_rel(uint32_t saddr, uint32_t v) {
   uint32_t old;
@@ -262,79 +271,47 @@ __device__ __forceinline__ uint32_t atom_add_acq_rel(uint32_t saddr, uint32_t v)
   return old;
 }
 
-// Refill of warpgroup wg's ring: load the warpgroup's halves of the next step of its Feed into ring slots n % 4 and
-// n % 4 + 1 (n: sequence number of the step's first slot) and advance the cursor by one step.  The single-pass engine
-// loads the W_hi slot only (the weight image stores every tile as hi, lo) and steps over W_lo.
-template <bool FAST>
-__device__ __forceinline__ void refill(uint32_t bar_base, uint32_t b_base, uint32_t n, int wg) {
-  Feed& f = feed(wg);
-  const uint8_t* src = f.src;
-  if (src == nullptr) return;
-  // every CTA streams the same 2 x 10 MB of weight images; keep them in L2 ahead of the projected maps that the
-  // gather streams past them (evict_first, stage_gather)
-  const uint64_t keep = f.keep;
-  const uint32_t sl = n % NSLOTS;
-#pragma unroll
-  for (uint32_t k = 0; k < (FAST ? 1u : 2u); ++k) {
-    const uint32_t full = bar_base + (BAR_FULL + sl + k) * 8;
-    mbar_expect_tx(full, HALF_SLOT_BYTES);
-    bulk_g2s_hint(b_base + (sl + k) * SLOT_BYTES, src + k * SLOT_BYTES, HALF_SLOT_BYTES, full, keep);
-  }
-  const int left = f.left - 1;
-  f.left = left;
-  if (left == 0)
-    f.next_run();
-  else
-    f.src = src + 2 * SLOT_BYTES;
-}
-
-// Weight rings: one per warpgroup.  Warpgroup g multiplies only rows [64g, 64g+64) of every 128-row weight tile, the
-// contiguous 8 KB at byte 8192 g of each 16 KB slot, so each warpgroup streams its own halves of the 4 slots
-// with its own FULL mbarriers, release counts and Feed cursor; the two rings share nothing.  The halves are filled in
-// exactly the order the warpgroup uses them; every step takes two consecutive slots (W_hi, W_lo of one 128-row x 64-k
-// tile), so steps alternate between slots 0-1 and 2-3.  A step's halves are released once the wgmma that read them
-// have completed: at the next step's acquire(), which retires the step (wait_group 0) and releases it BEFORE it waits
-// for the next step's slots, or at the drain that ends an MMA run.  Each warp's lane 0 releases a step with an
-// acq_rel atomic add on the count of its slot pair, and the warp whose add completes the step's 4 releases (old count
-// 3 mod 4) refills the pair at once with the step two ahead: nobody waits to refill.  So while a warpgroup waits for
-// step s + 1 to land, the copy of step s + 2 is already in flight beside it; releasing s only after s + 1 had landed
-// and been issued (wait_group 1 after the commit of s + 1) left one copy in flight per warpgroup, and the step period
-// was a whole L2 -> shared-memory round trip.  Steps 0 and 1 are loaded at kernel start.  A warpgroup never waits for
-// the other one's refill, so the two may drift apart by up to a step between two workers_sync, which staggers their
-// use of the tensor pipe and of L2; while one warpgroup waits for its step to retire, the other's wgmma keep the
-// tensor pipe busy.
-//  * The count needs no reset: a warp releases step s + 2 (same slot pair) only after its FULL wait for s + 2, whose
-//    load the last release of step s issued, so the 4 releases of one step are the 4 consecutive adds on their count.
-//  * No slot is freed under a reader: the release follows wait_group 0, when every wgmma of the warp's warpgroup that
-//    read the step has completed.  Every warp runs the same wait_group sequence (none depends on data).
-//  * Refills stay in slot order: each warp releases every step once and in step order, and releases step s + 1 only
-//    after the refill it may have done at its release of s has returned, so the refill at the last release of s + 1
-//    follows the refill of s.
-//  * Cursor visibility: the Feed writes of one refill happen before the refilling warp's release add of the next step
-//    on the other count, which the next refiller's add reads (acquire): the next refill sees the cursor advanced.
-//  * Pass change: the cursor runs on into the next pass's weight image, so the releases of the coarse pass's last two
-//    steps (at the drains that end the pass) load the fine pass's first two, which arrive during the flush and the
-//    `ready` wait.
-// There is no wait on the refill path, so nothing to deadlock on; only acquire() waits, on FULL, after its own warp
-// has released every earlier step (the other warps release theirs without waiting for anything).
+// Weight rings: one per consumer warpgroup.  Warpgroup g multiplies only rows [64g, 64g+64) of every 128-row weight
+// tile, the contiguous 8 KB at byte 8192 g of each 16 KB slot, so each warpgroup has its own halves of the 4 slots
+// with its own FULL mbarriers and release counts, and its own producer lane (produce()); the two rings share nothing.
+// The halves are filled in exactly the order the warpgroup uses them; every step takes two consecutive slots (W_hi,
+// W_lo of one 128-row x 64-k tile), so steps alternate between slots 0-1 and 2-3.  A step's halves are released once
+// the wgmma that read them have completed: at the next step's acquire(), which retires the step (wait_group 0) and
+// releases it BEFORE it waits for the next step's slots, or at the drain that ends an MMA run.  Each warp's lane 0
+// releases a step with an acq_rel atomic add on the count of its slot pair; that is all the consumers do for the
+// ring.  The producer lane of the ring issues steps 0 and 1 at kernel start and step s + 2 as soon as the count of
+// s's slot pair shows all 4 releases of s, so while a warpgroup waits for step s + 1 to land, the copy of s + 2 is
+// already in flight beside it.  A warpgroup never waits for the other one's ring, so the two may drift apart by up to
+// a step between two workers_sync, which staggers their use of the tensor pipe and of L2.
+//  * The count needs no reset: a warp releases step s + 2 (same slot pair) only after its FULL wait for s + 2, which
+//    the producer issued only after the 4 releases of s, so the 4 releases of one step are the 4 consecutive adds on
+//    their count and the count reaches 4 (s / 2 + 1) exactly when step s is released.
+//  * No slot is freed under a reader: the producer issues s + 2 only after all 4 releases of s (its acquire load
+//    reads the last of the acq_rel adds), and each release follows wait_group 0, when every wgmma of the warp's
+//    warpgroup that read the step has completed.  Every warp runs the same wait_group sequence (none depends on data).
+//  * Slot order: one lane issues a ring's refills, in sequence order.
+//  * No deadlock: the producer waits only for the releases of step s, which every warp makes before any wait other than
+//    the FULL wait of step s + 1 (issued before), since every MMA run ends with a drain before workers_sync, the flush
+//    and the fine pass's `ready` wait.  So the producer never waits for anything that those can block.
+//  * Pass change: the sequence runs on into the next pass's weight image, so the releases of the coarse pass's last
+//    two steps (at the drains that end the pass) let the producer load the fine pass's first two, which arrive during
+//    the flush and the `ready` wait.
 // FAST (single-pass engine): the same sequence numbers and the same protocol on each step's first (W_hi) slot only;
 // the barriers of the W_lo slots are never used.
 template <bool FAST>
 struct Ring {
-  uint32_t bar_base, b_base;   // this warpgroup's barriers; its half of slot 0
+  uint32_t bar_base, b_base;   // this warpgroup's ring control (barriers, release counts); its half of slot 0
   uint32_t seq;      // slot sequence number of the next step
-  uint32_t pend;     // first slot of the step still in flight (valid if has_pend)
-  bool has_pend;
-  int lane;
+  bool has_pend;     // step seq - 2 is still in flight
   int* status;
   __device__ __forceinline__ uint32_t slot_addr(uint32_t s) const { return b_base + (s % NSLOTS) * SLOT_BYTES; }
-  // retire and release the step before (its refill leaves now), then wait for this step's slots
+  // retire and release the step before (the producer refills its slots), then wait for this step's slots
   __device__ __forceinline__ void acquire() {
     if (has_pend) {
       PROF_BEGIN(t1);
       wgmma_wait<0>();
       PROF_END(PH_WGMMA_WAIT, t1);
-      release(pend);
+      release(seq - 2);
       has_pend = false;
     }
     PROF_BEGIN(t0);
@@ -345,20 +322,12 @@ struct Ring {
   }
   __device__ __forceinline__ void release(uint32_t s) {
     __syncwarp();
-    if (lane == 0) {
-      const int wg = threadIdx.x >> 7;
-      if (atom_add_acq_rel(smem_u32(&feed(wg).released[(s / 2) & 1]), 1) % 4 == 3) {
-        PROF_BEGIN(t0);
-        refill<FAST>(bar_base, b_base, s + NSLOTS, wg);
-        PROF_END_ANY(PH_REFILL, t0);
-      }
-    }
+    if ((threadIdx.x & 31) == 0) atom_add_acq_rel(bar_base + RING_RELEASED + ((s / 2) & 1) * 4, 1);
     __syncwarp();
   }
   // after the step's wgmma are issued: commit them as one group (the next acquire() or drain() retires it)
   __device__ __forceinline__ void issued() {
     wgmma_commit();
-    pend = seq;
     has_pend = true;
     seq += 2;
   }
@@ -366,10 +335,44 @@ struct Ring {
     PROF_BEGIN(t0);
     wgmma_wait<0>();
     PROF_END(PH_WGMMA_WAIT, t0);
-    if (has_pend) release(pend);
+    if (has_pend) release(seq - 2);
     has_pend = false;
   }
 };
+
+// The producer lane of ring g (lane 0 of warp 8 + g): loads ring g's halves of steps 0 and 1, then of each step
+// s + 2 once the 4 warps of consumer warpgroup g have released step s, into ring slots (2 s) % 4 and (2 s) % 4 + 1.
+// It walks on to the next step's source right after each issue, so the copy leaves as soon as the count completes.
+// The single-pass engine loads the W_hi slot only (the weight image stores every tile as hi, lo) and steps over W_lo.
+template <bool FAST>
+__device__ __forceinline__ void produce(const Params& p, int g) {
+  const uint32_t bar_base = smem_u32(smem + SM_BAR) + g * RING_BYTES;
+  const uint32_t b_base = smem_u32(smem + SM_B) + g * HALF_SLOT_BYTES;
+  // every CTA streams the same 2 x 10 MB of weight images; keep them in L2 ahead of the projected maps that the
+  // gather streams past them (evict_first, stage_gather)
+  uint64_t keep;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(keep));
+  Feed f;
+  f.tile = blockIdx.x >> 1;
+  f.ps = 0;
+  f.v = 0;
+  f.begin_run(p, g);
+  PROF_SUM_INIT(t_refill);
+  for (uint32_t s = 0; f.src != nullptr; ++s) {
+    const uint32_t pair = s & 1;
+    if (s >= 2) wait_count(bar_base + RING_RELEASED + pair * 4, 4 * (s >> 1), p.status, 220 + 2 * g + (int)pair);
+    PROF_BEGIN(t0);
+#pragma unroll
+    for (uint32_t k = 0; k < (FAST ? 1u : 2u); ++k) {
+      const uint32_t full = bar_base + (BAR_FULL + 2 * pair + k) * 8;
+      mbar_expect_tx(full, HALF_SLOT_BYTES);
+      bulk_g2s_hint(b_base + (2 * pair + k) * SLOT_BYTES, f.src + k * SLOT_BYTES, HALF_SLOT_BYTES, full, keep);
+    }
+    PROF_SUM(t_refill, t0);
+    f.next(p, g);
+  }
+  PROF_PUBLISH(p.status, PH_REFILL, t_refill);
+}
 
 // acc (+)= A[64 x 16 KSTEPS] * W^T over one step: Ahi*Whi + Alo*Whi + Ahi*Wlo (FAST: Ahi*Whi only)
 template <bool FAST, int KSTEPS>
@@ -698,8 +701,9 @@ __device__ __forceinline__ void field_tc(const Params& p) {
   const int rank = blockIdx.x & 1;        // which 64 points of the 128-point tile
   const int pair = blockIdx.x >> 1;
   const int n_pairs = gridDim.x >> 1;
-  const int wg = threadIdx.x >> 7;
-  const uint32_t bar_base = smem_u32(smem + SM_BAR) + wg * BAR_COUNT * 8;   // this warpgroup's ring
+  const int wg = threadIdx.x >> 7;        // consumer warpgroups 0-1; 2: the producer
+  const bool producer = wg == 2;
+  const uint32_t bar_base = smem_u32(smem + SM_BAR) + wg * RING_BYTES;   // this warpgroup's ring
   const uint32_t b_base = smem_u32(smem + SM_B) + wg * HALF_SLOT_BYTES;
   int* n_list = reinterpret_cast<int*>(smem + SM_NLIST);
   const int NS = p.sc.NS;
@@ -707,32 +711,22 @@ __device__ __forceinline__ void field_tc(const Params& p) {
   PROF_BEGIN(t_kernel);
   PROF_INIT();
 
-  if ((threadIdx.x & 127) == 0) {
+  if (!producer && (threadIdx.x & 127) == 0) {
     for (int i = 0; i < NSLOTS; ++i) mbar_init(bar_base + (BAR_FULL + i) * 8, 1);
     if (threadIdx.x == 0) *n_list = 0;
-    Feed& f = feed(wg);
-    for (int i = 0; i < 2; ++i) {
-      f.slots[i] = i < p.npass ? p.pass[i].packed + HEADER_BYTES + wg * HALF_SLOT_BYTES : nullptr;
-      f.n_tiles[i] = i < p.npass ? p.pass[i].n_tiles : 0;
-    }
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(f.keep));
-    f.released[0] = f.released[1] = 0;
-    f.npass = p.npass;
-    f.NS = NS;
-    f.pair = pair;
-    f.n_pairs = n_pairs;
-    f.ps = 0;
-    f.v = 0;
-    f.tile = pair;
-    f.begin_run();
+    uint32_t* released = reinterpret_cast<uint32_t*>(smem + SM_BAR + wg * RING_BYTES + RING_RELEASED);
+    released[0] = released[1] = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if ((threadIdx.x & 127) == 0) {
-    // prefill: steps 0 and 1
-    refill<FAST>(bar_base, b_base, 0, wg);
-    refill<FAST>(bar_base, b_base, 2, wg);
+  // ptxas allocates each side for the budget its setmaxnreg sets, as long as the two paths never join again
+  if (producer) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    // lane 0 of producer warp g refills ring g; the rest of the producer warpgroup has nothing to do
+    if (lane == 0 && warp < NCONSUMER_WARPS + 2) produce<FAST>(p, warp - NCONSUMER_WARPS);
+    return;
   }
+  setmaxnreg_inc<CONSUMER_REGS>();
   const size_t map_stride = (size_t)p.sc.SB * NS * p.sc.Hl * p.sc.Wl * D;
 
   {
@@ -748,9 +742,7 @@ __device__ __forceinline__ void field_tc(const Params& p) {
     rg.bar_base = bar_base;
     rg.b_base = b_base;
     rg.seq = 0;
-    rg.pend = 0;
     rg.has_pend = false;
-    rg.lane = lane;
     rg.status = p.status;
     float x[4][32];
     float* scratch = p.scratch + (size_t)blockIdx.x * D * ROWS;

@@ -7,11 +7,12 @@ namespace pnr {
 namespace tcptx {
 
 constexpr long long TIMEOUT_CYCLES = 4000000000LL;  // ~2 s: turns a protocol bug into an error, not a hang
+constexpr long long TIMEOUT_NS = 2000000000LL;      // the same on the global timer
 // status[20] multiplies the limit (PNR_TC_TIMEOUT_MULT; profilers that replay with heavy instrumentation slow a launch
 // down by two orders of magnitude)
-__device__ __forceinline__ long long timeout_limit(const int* status) {
+__device__ __forceinline__ long long timeout_limit(const int* status, long long base = TIMEOUT_CYCLES) {
   const int m = ((const volatile int*)status)[20];
-  return TIMEOUT_CYCLES * (long long)(m > 1 ? m : 1);
+  return base * (long long)(m > 1 ? m : 1);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -39,6 +40,11 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity)
       : "memory");
   return ok;
 }
+__device__ __forceinline__ uint32_t ld_acquire_shared(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(saddr) : "memory");
+  return v;
+}
 static __device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity, int* status, int tag) {
   long long t0 = clock64();
   uint32_t spins = 0;
@@ -58,6 +64,35 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* st
   mbar_wait_slow(bar, parity, status, tag);
 }
 
+// Wait until the u32 at saddr reaches target (acquire: what the threads that counted it up did before is visible),
+// polling with __nanosleep back-off; the same status / tag / trap protocol as mbar_wait.  This slow path runs in a
+// warpgroup with a small setmaxnreg budget, which cannot call mbar_wait_slow (ptxas allocates a subroutine for one
+// budget), and it measures its limit on the global timer.
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+static __device__ __noinline__ void wait_count_slow(uint32_t saddr, uint32_t target, int* status, int tag) {
+  const unsigned long long t0 = globaltimer_ns();
+  uint32_t spins = 0;
+  while (ld_acquire_shared(saddr) < target) {
+    __nanosleep(20);
+    if ((++spins & 0xFF) == 0) {
+      if (*(volatile int*)status != 0) return;
+      if (globaltimer_ns() - t0 > (unsigned long long)timeout_limit(status, TIMEOUT_NS)) {
+        atomicCAS(status, 0, tag);
+        if (((volatile int*)status)[1]) __trap();
+        return;
+      }
+    }
+  }
+}
+__device__ __forceinline__ void wait_count(uint32_t saddr, uint32_t target, int* status, int tag) {
+  if (ld_acquire_shared(saddr) >= target) return;
+  wait_count_slow(saddr, target, status, tag);
+}
+
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                "l"(src), "r"(bytes), "r"(bar)
@@ -73,6 +108,17 @@ __device__ __forceinline__ void bulk_g2s_hint(uint32_t dst, const void* src, uin
 }
 // generic-proxy shared-memory writes (operand tiles) become visible to the async proxy (wgmma)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// Per-warpgroup register budget (warp-specialised kernels): every warp of the warpgroup executes it.  dec hands
+// registers back to the CTA's pool, inc waits until the pool can grant the new count.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 
 // ---------------------------------------------------------------------------------------
 // wgmma (warpgroup MMA): D[64 x N] (+)= A[smem desc] * B[smem desc]^T, fp32 accumulators in registers.

@@ -5,13 +5,12 @@ Loads the profile build of the library (`make -C pixel-nerf_b200/csrc prof` -> l
 -DPNR_TC_PROFILE), renders full frames of bench.py's C2, C3 and C4 rays with the exact ("tc") and the single-pass
 ("tc_fast") engine, and reads the kernel's 8 phase counters (pnr_tc_counters): clock64() time the first thread of each
 warpgroup spent waiting on a weight slot (FULL), in wgmma_wait (retiring the previous step with wait_group 0 before
-the next step's FULL wait, and the drains that end an MMA run), in the 256-thread barrier, gathering the projected
-latent, in geometry and the fine pass's `ready` poll, finishing rays (flush), and in all; and the time the ring's
-refills took, counted on whichever warp's lane 0 released a step last and so issued its refill (that release now
-comes right after the retire wait, before the FULL wait).  They are printed as
-SM clocks per weight step (a step is one 64-wide k-chunk of 128 weight rows: 9 or 12 wgmma per warpgroup); "other" is
-the total less the other phases (wgmma issue, epilogue arithmetic; the refills that the first thread did not issue are
-subtracted as well, though they ran on other warps).  Each
+the next step's FULL wait, and the drains that end an MMA run), in the 256-thread barrier of the consumers, gathering
+the projected latent, in geometry and the fine pass's `ready` poll, finishing rays (flush), and in all; and the time
+the ring's refills took to issue, counted on the producer lane of each ring (not the time it waits for releases).
+They are printed as SM clocks per weight step (a step is one 64-wide k-chunk of 128 weight rows: 9 or 12 wgmma per
+warpgroup); "other" is the first thread's total less its own phases (wgmma issue, epilogue arithmetic); the refills
+run on the producer warpgroup beside them and are not subtracted.  Each
 line names the card, its power limit and the SM clock sampled during the frames.  The counters change the timing a
 little; the production library is timed by bench.py.
 
@@ -118,7 +117,7 @@ def main():
                    "clock_reasons": clk.get("reasons")}
             if cnt[-1] > 0:
                 cps = {name: c / per for name, c in zip(PHASES, cnt)}
-                cps["other"] = cps["total"] - sum(cps[n] for n in PHASES[:-1])
+                cps["other"] = cps["total"] - sum(cps[n] for n in PHASES[:-1] if n != "refill")
                 res["clocks_per_step"] = {k: round(v, 1) for k, v in cps.items()}
             print(json.dumps(res), flush=True)
             if args.dump:

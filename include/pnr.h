@@ -463,7 +463,7 @@ int pnr_grid_points(const double* lo, const double* hi, const int32_t* reso, int
  * (grid point, axis) order and shared by every cell touching the edge (the mesh is welded), at the lower corner's grid
  * index plus t = (iso - s_a) / (s_b - s_a) along the edge in float64 (0.5 when the outside corner is NaN or infinite).  Triangles
  * come from generated tables (oracle/make_mc_tables.py), cells in linear order, counter-clockwise seen from outside
- * the inside region (normals toward decreasing sigma); every face is resolved from its own four corners, so the
+ * the inside region (normals toward decreasing sigma; pnr_mc_vertex_attrs gives per-vertex ones); every face is resolved from its own four corners, so the
  * surface is watertight.  Offsets are exclusive scans (no atomics): repeated calls give the same bits.
  * A dimension below 2 gives no cells, vertices or triangles.  Errors: dimensions < 1 or above 2^36 points, negative
  * sizes, NULL pointers -> PNR_ERR_INVALID; workspace < pnr_mc_workspace_bytes -> PNR_ERR_WORKSPACE. */
@@ -472,6 +472,27 @@ int pnr_mc_count(const float* vol, int32_t nx, int32_t ny, int32_t nz, double is
                  void* workspace, size_t workspace_bytes, void* stream);
 int pnr_mc_emit(const float* vol, int32_t nx, int32_t ny, int32_t nz, double iso, double* verts, int64_t* tris,
                 int64_t n_verts, int64_t n_tris, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Per-vertex attributes of the mesh pnr_mc_emit writes (call it after pnr_mc_count on the same stream, with the same
+ * vol / dims / iso / workspace); attribute i belongs to vertex i.  lo, hi: HOST double[3], the bounds the grid spans
+ * (pnr_grid_points' lo / hi), h_k = (hi_k - lo_k) / (n_k - 1).  All in float64 with round-to-nearest intrinsics, no
+ * atomics: repeated calls give the same bits.
+ *   normals  [n_verts][3] float64: -G / |G|, toward decreasing sigma (the side the winding faces).  G is the grid
+ *            gradient of sigma at the edge's corners a, b, interpolated as (1 - t) g(a) + t g(b) with the vertex's t,
+ *            then divided by h_k.  Per axis at a grid point, g is the central difference where both neighbours exist
+ *            and are finite, else the forward, else the backward difference where the point and that neighbour are
+ *            finite, else 0, so a non-finite sigma never spreads into its neighbours.  |G|^2 = (Gx^2 + Gy^2) + Gz^2;
+ *            where |G| is 0 or not finite, the unit vector along the edge from its inside corner to its outside one.
+ *   xyz      [n_verts][3] fp32: the vertex's world position lo + v h (v its index coordinate), with pnr_grid_points'
+ *            bits on grid indices.  This is where the surface is, unlike recon.py's returned vertices, which keep the
+ *            reference's (c2 - c1) / reso scale.
+ *   viewdirs [n_verts][3] fp32: -normal, a camera facing the surface head-on from outside.
+ * Any output may be NULL.  A dimension below 2 returns PNR_OK without writing.  Errors: dimensions < 1 or above 2^36
+ * points, negative n_verts, NULL vol / lo / hi -> PNR_ERR_INVALID; workspace < pnr_mc_workspace_bytes ->
+ * PNR_ERR_WORKSPACE. */
+int pnr_mc_vertex_attrs(const float* vol, int32_t nx, int32_t ny, int32_t nz, double iso, const double* lo,
+                        const double* hi, double* normals, float* xyz, float* viewdirs, int64_t n_verts,
+                        void* workspace, size_t workspace_bytes, void* stream);
 
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.

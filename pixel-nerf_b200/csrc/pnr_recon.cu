@@ -195,6 +195,87 @@ __global__ void k_mc_verts(const float* __restrict__ vol, int nx, int ny, int nz
   }
 }
 
+// ---- vertex attributes ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool finite_f32(float v) { return fabsf(v) <= 3.402823466e38f; }
+
+// axis k of the sigma gradient at grid point p (index i of n along the axis), in index units: the central difference
+// where both neighbours exist and are finite, else a one-sided difference with a finite centre, else 0.  A NaN (the
+// grid origin, whose fake view direction is 0 / 0) or an infinity never reaches a neighbour's gradient.
+__device__ __forceinline__ double grid_grad(const float* __restrict__ vol, int64_t p, int i, int n, int64_t step) {
+  const bool up = i + 1 < n, dn = i > 0;
+  const float c = vol[p], su = up ? vol[p + step] : 0.0f, sd = dn ? vol[p - step] : 0.0f;
+  if (up && dn && finite_f32(su) && finite_f32(sd)) return __ddiv_rn(__dsub_rn((double)su, (double)sd), 2.0);
+  if (up && finite_f32(c) && finite_f32(su)) return __dsub_rn((double)su, (double)c);
+  if (dn && finite_f32(c) && finite_f32(sd)) return __dsub_rn((double)c, (double)sd);
+  return 0.0;
+}
+
+// lo + v * h for an index coordinate v of an axis of n >= 2 points; on a grid index the bits of linspace_f32
+__device__ __forceinline__ float index_to_world_f32(double lo, double hi, int n, double v) {
+  const int i = (int)v;
+  if ((double)i == v) return linspace_f32(lo, hi, n, i);
+  const double h = __ddiv_rn(__dsub_rn(hi, lo), (double)(n - 1));
+  return __double2float_rn(__dadd_rn(__dmul_rn(v, h), lo));
+}
+
+// per vertex of k_mc_verts (same edges, same ids, same t): the unit normal -G/|G| from the grid gradient interpolated
+// along the edge, G in world units (toward decreasing sigma; along the edge from its inside corner to its outside
+// corner where |G| is 0 or not finite), the vertex's world position, and the view direction -normal
+__global__ void k_mc_vertex_attrs(const float* __restrict__ vol, int nx, int ny, int nz, double iso, double lo0,
+                                  double lo1, double lo2, double hi0, double hi1, double hi2,
+                                  const uint8_t* __restrict__ flags, const int64_t* __restrict__ vid, int64_t n_verts,
+                                  double* __restrict__ normals, float* __restrict__ xyz,
+                                  float* __restrict__ viewdirs) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t N = (int64_t)nx * ny * nz;
+  if (p >= N) return;
+  const int z = (int)(p % nz);
+  const int y = (int)((p / nz) % ny);
+  const int x = (int)(p / ((int64_t)ny * nz));
+  const int64_t step[3] = {(int64_t)ny * nz, (int64_t)nz, 1};
+  const int dim[3] = {nx, ny, nz};
+  const double lo[3] = {lo0, lo1, lo2}, hi[3] = {hi0, hi1, hi2};
+  double ga[3];
+  bool have_ga = false;
+  for (int a = 0; a < 3; ++a) {
+    if (!flags[p * 3 + a]) continue;
+    const int64_t id = vid[p * 3 + a];
+    if (id >= n_verts) continue;
+    const float sa = vol[p], sb = vol[p + step[a]];
+    double t = 0.5;                       // as k_mc_verts computes it
+    if (finite_f32(sa) && finite_f32(sb))
+      t = __ddiv_rn(__dsub_rn(iso, (double)sa), __dsub_rn((double)sb, (double)sa));
+    int ia[3] = {x, y, z}, ib[3] = {x, y, z};
+    ib[a] += 1;
+    if (!have_ga) {
+      for (int k = 0; k < 3; ++k) ga[k] = grid_grad(vol, p, ia[k], dim[k], step[k]);
+      have_ga = true;
+    }
+    double G[3], h[3];
+    for (int k = 0; k < 3; ++k) {
+      const double gb = grid_grad(vol, p + step[a], ib[k], dim[k], step[k]);
+      h[k] = __ddiv_rn(__dsub_rn(hi[k], lo[k]), (double)(dim[k] - 1));
+      G[k] = __ddiv_rn(__dadd_rn(__dmul_rn(__dsub_rn(1.0, t), ga[k]), __dmul_rn(t, gb)), h[k]);
+    }
+    // the double-precision sqrt is IEEE round-to-nearest on the GPU (as __dsqrt_rn) and in numpy
+    const double len =
+        sqrt(__dadd_rn(__dadd_rn(__dmul_rn(G[0], G[0]), __dmul_rn(G[1], G[1])), __dmul_rn(G[2], G[2])));
+    double nrm[3] = {0.0, 0.0, 0.0};
+    if (len > 0.0 && len <= 1.7976931348623157e308) {
+      for (int k = 0; k < 3; ++k) nrm[k] = __ddiv_rn(-G[k], len);
+    } else {
+      nrm[a] = (mc_inside(sa, iso) != (h[a] < 0.0)) ? 1.0 : -1.0;
+    }
+    double v[3] = {(double)x, (double)y, (double)z};     // the vertex of k_mc_verts, in index units
+    v[a] = __dadd_rn(v[a], t);
+    for (int k = 0; k < 3; ++k) {
+      if (normals) normals[id * 3 + k] = nrm[k];
+      if (xyz) xyz[id * 3 + k] = index_to_world_f32(lo[k], hi[k], dim[k], v[k]);
+      if (viewdirs) viewdirs[id * 3 + k] = __double2float_rn(-nrm[k]);
+    }
+  }
+}
+
 // the triangles of each cell in table order at the cell's scanned offset, as vertex ids of their edges
 __global__ void k_mc_tris(int nx, int ny, int nz, const uint8_t* __restrict__ cube,
                           const int64_t* __restrict__ toff, const int64_t* __restrict__ vid, int64_t n_tris,
@@ -341,6 +422,29 @@ int pnr_mc_emit(const float* vol, int32_t nx, int32_t ny, int32_t nz, double iso
     k_mc_tris<<<blocks, kPtThreads, 0, s>>>(nx, ny, nz, w.cube, w.toff, w.vid, n_tris, tris);
     PNR_LAUNCH_CHECK();
   }
+  return PNR_OK;
+}
+
+int pnr_mc_vertex_attrs(const float* vol, int32_t nx, int32_t ny, int32_t nz, double iso, const double* lo,
+                        const double* hi, double* normals, float* xyz, float* viewdirs, int64_t n_verts,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_dims(nx, ny, nz);
+  if (rc) return rc;
+  PNR_CHECK_ARG(n_verts >= 0, "negative n_verts");
+  PNR_CHECK_ARG(lo && hi, "NULL bounds");
+  if (nx < 2 || ny < 2 || nz < 2) return PNR_OK;
+  PNR_CHECK_ARG(vol != nullptr, "NULL volume");
+  const int64_t N = (int64_t)nx * ny * nz;
+  McWs w;
+  const size_t need = mc_carve(N, workspace, workspace_bytes, &w);
+  if (workspace == nullptr || workspace_bytes < need) {
+    set_error("workspace too small: %zu < %zu", workspace_bytes, need);
+    return PNR_ERR_WORKSPACE;
+  }
+  if (n_verts == 0 || (!normals && !xyz && !viewdirs)) return PNR_OK;
+  k_mc_vertex_attrs<<<(unsigned)((N + kPtThreads - 1) / kPtThreads), kPtThreads, 0, (cudaStream_t)stream>>>(
+      vol, nx, ny, nz, iso, lo[0], lo[1], lo[2], hi[0], hi[1], hi[2], w.flags, w.vid, n_verts, normals, xyz, viewdirs);
+  PNR_LAUNCH_CHECK();
   return PNR_OK;
 }
 

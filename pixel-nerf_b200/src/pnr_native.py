@@ -166,7 +166,8 @@ def declare(L):
         L.pnr_mc_workspace_bytes.restype = sz
         L.pnr_mc_count.argtypes = [vp, i32, i32, i32, f64, vp, vp, sz, vp]
         L.pnr_mc_emit.argtypes = [vp, i32, i32, i32, f64, vp, vp, i64, i64, vp, sz, vp]
-        for name in ("pnr_grid_points", "pnr_mc_count", "pnr_mc_emit"):
+        L.pnr_mc_vertex_attrs.argtypes = [vp, i32, i32, i32, f64, P(f64), P(f64), vp, vp, vp, i64, vp, sz, vp]
+        for name in ("pnr_grid_points", "pnr_mc_count", "pnr_mc_emit", "pnr_mc_vertex_attrs"):
             getattr(L, name).restype = C.c_int
     L.pnr_set_deterministic.argtypes = [C.c_int]
     L.pnr_set_deterministic.restype = C.c_int
@@ -323,9 +324,11 @@ def grid_points(lo, hi, reso, first, count, xyz, viewdirs=None):
                                     dptr(viewdirs, "viewdirs"), stream_ptr(dev)))
 
 
-def marching_cubes(vol, iso):
+def marching_cubes(vol, iso, *, bounds=None):
     """pnr_mc_count + pnr_mc_emit on a contiguous fp32 CUDA volume (nx, ny, nz) -> (vertices float64 [N, 3] in grid
-    index space, triangles int64 [M, 3]), CUDA tensors on vol's device.  Synchronises once, to size the outputs."""
+    index space, triangles int64 [M, 3]), CUDA tensors on vol's device.  Synchronises once, to size the outputs.
+    With bounds = (lo, hi), the world box the grid spans, pnr_mc_vertex_attrs also runs and the result is
+    (vertices, triangles, normals float64 [N, 3], xyz float32 [N, 3], viewdirs float32 [N, 3])."""
     if vol.dim() != 3:
         raise RuntimeError(f"marching_cubes: expected a 3-D volume, got shape {tuple(vol.shape)}")
     nx, ny, nz = vol.shape
@@ -342,7 +345,16 @@ def marching_cubes(vol, iso):
         tris = torch.empty(nt, 3, dtype=torch.int64, device=dev)
         check(L.pnr_mc_emit(dptr(vol, "vol"), nx, ny, nz, float(iso), C.c_void_p(verts.data_ptr()),
                             C.c_void_p(tris.data_ptr()), nv, nt, C.c_void_p(ws.data_ptr()), ws.numel(), s))
-    return verts, tris
+        if bounds is None:
+            return verts, tris
+        lo, hi = bounds
+        normals = torch.empty(nv, 3, dtype=torch.float64, device=dev)
+        xyz = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+        viewdirs = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+        check(L.pnr_mc_vertex_attrs(dptr(vol, "vol"), nx, ny, nz, float(iso), (C.c_double * 3)(*map(float, lo)),
+                                    (C.c_double * 3)(*map(float, hi)), C.c_void_p(normals.data_ptr()), dptr(xyz),
+                                    dptr(viewdirs), nv, C.c_void_p(ws.data_ptr()), ws.numel(), s))
+    return verts, tris, normals, xyz, viewdirs
 
 
 def profile_begin():

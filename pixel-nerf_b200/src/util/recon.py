@@ -3,7 +3,8 @@ Mesh reconstruction tools (the reference's src/util/recon.py), on the GPU.
 
 `marching_cubes` evaluates sigma on a grid with the fused field kernels and extracts the isosurface with the
 library's own marching cubes (`pnr_grid_points`, `pnr_field_eval`, `pnr_mc_count` / `pnr_mc_emit`, include/pnr.h):
-the grid, the sigma volume and the mesh stay on the device, and only the mesh comes back.  There is no CPU path.
+the grid, the sigma volume and the mesh stay on the device, and only the mesh comes back.  With `return_colors`,
+`pnr_mc_vertex_attrs` adds normals and the field colours each vertex.  There is no CPU path.
 """
 import warnings
 
@@ -23,6 +24,7 @@ def marching_cubes(
     eval_batch_size=100000,
     coarse=True,
     device=None,
+    return_colors=False,
 ):
     """
     Run marching cubes on network.
@@ -38,8 +40,13 @@ def marching_cubes(
     :param coarse whether to use coarse NeRF for evaluation
     :param device optionally, device to put points for evaluation.
     By default uses device of occu_net's first parameter.
+    :param return_colors also return per-vertex normals and colours (pnr_mc_vertex_attrs, then the field at each
+    vertex)
     :return vertices (N, 3) float64 numpy, scaled as vertex index * (c2 - c1) / reso + c1; triangles (M, 3) int64
-    numpy of vertex ids, counter-clockwise seen from outside (normals toward decreasing sigma)
+    numpy of vertex ids, counter-clockwise seen from outside (normals toward decreasing sigma).  With return_colors,
+    also normals (N, 3) float64 numpy, unit, toward decreasing sigma (from the sigma grid's gradient), and rgb (N, 3)
+    float32 numpy: channels 0-2 of occu_net at the vertex's true position on the surface, seen head-on from outside
+    (view direction -normal), in eval_batch_size chunks with occu_net's engine
     """
     if occu_net.use_viewdirs:
         warnings.warn(
@@ -70,7 +77,19 @@ def marching_cubes(
                 sigmas[first:first + n] = out[0, :, sigma_idx]
 
             print("Running marching cubes")
-            vertices, triangles = pn.marching_cubes(sigmas.view(*reso), isosurface)
+            if not return_colors:
+                vertices, triangles = pn.marching_cubes(sigmas.view(*reso), isosurface)
+            else:
+                # the field is queried where the surface is (xyz), not at the returned vertices, which keep the
+                # reference's (c2 - c1) / reso scale below
+                vertices, triangles, normals, xyz, vd = pn.marching_cubes(sigmas.view(*reso), isosurface,
+                                                                          bounds=(c1, c2))
+                print("Evaluating colour @", len(xyz), "vertices")
+                rgb = torch.empty(len(xyz), 3, dtype=torch.float32, device=device)
+                for first in range(0, len(xyz), bs):
+                    out = occu_net(xyz[None, first:first + bs], coarse=coarse, viewdirs=vd[None, first:first + bs])
+                    rgb[first:first + bs] = out[0, :, :3]
+                normals, rgb = normals.cpu().numpy(), rgb.cpu().numpy()
             vertices, triangles = vertices.cpu().numpy(), triangles.cpu().numpy()
     finally:
         if is_train:
@@ -78,20 +97,29 @@ def marching_cubes(
     # Scale (by reso, not reso - 1, as the reference does)
     c1, c2 = np.array(c1), np.array(c2)
     vertices *= (c2 - c1) / np.array(reso)
+    if return_colors:
+        return vertices + c1, triangles, normals, rgb
     return vertices + c1, triangles
 
 
-def save_obj(vertices, triangles, path, vert_rgb=None):
+def save_obj(vertices, triangles, path, vert_rgb=None, vert_normals=None):
     """
-    Save an OBJ file: one `v x y z` line per vertex (`v x y z r g b` with per-vertex colours), then one 1-based
-    `f a b c` line per triangle; every coordinate and colour with %.4f.
+    Save an OBJ file: one `v x y z` line per vertex (`v x y z r g b` with per-vertex colours), then with normals one
+    `vn x y z` line per vertex, then one 1-based `f a b c` line per triangle (`f a//a b//b c//c` with normals); every
+    coordinate, colour and normal component with %.4f.
     :param vertices (N, 3)
     :param triangles (M, 3) 0-based vertex ids
     :param vert_rgb (N, 3) rgb, optional
+    :param vert_normals (N, 3) normals, optional
     """
     vertices = np.asarray(vertices)
     rows = vertices if vert_rgb is None else np.concatenate([vertices, np.asarray(vert_rgb)], axis=1)
     vfmt = "v" + " %.4f" * rows.shape[1] + "\n"
     with open(path, "w") as f:
         f.writelines(vfmt % tuple(r) for r in rows)
-        f.writelines("f %d %d %d\n" % (a + 1, b + 1, c + 1) for a, b, c in np.asarray(triangles))
+        if vert_normals is None:
+            f.writelines("f %d %d %d\n" % (a + 1, b + 1, c + 1) for a, b, c in np.asarray(triangles))
+        else:
+            f.writelines("vn %.4f %.4f %.4f\n" % tuple(n) for n in np.asarray(vert_normals))
+            f.writelines("f %d//%d %d//%d %d//%d\n" % (a + 1, a + 1, b + 1, b + 1, c + 1, c + 1)
+                         for a, b, c in np.asarray(triangles))

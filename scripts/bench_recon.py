@@ -4,9 +4,14 @@ synth.bench_mlp_weights, tensor engine): device time of the sigma grid (pnr_grid
 eval_batch_size points, as util.recon runs it) and of marching cubes (pnr_mc_count, the count download, pnr_mc_emit)
 at 128^3 and 256^3.  Prints one JSON line with the GPU's name and power limit.
 
-    python scripts/bench_recon.py [--reso 128 256] [--reps 5]
+With --colors it also times what return_colors=True adds: one pnr_mc_vertex_attrs launch (normals, query points and
+view directions of every vertex) and the field evaluation at the vertices (chunks of eval_batch_size, as util.recon
+runs it), both in device ms, with the vertex count.
+
+    python scripts/bench_recon.py [--reso 128 256] [--reps 5] [--engine tc] [--colors]
 """
 import argparse
+import ctypes as C
 import json
 import os
 import subprocess
@@ -52,6 +57,39 @@ def sigma_grid(net, c1, c2, reso, bs):
     return sig.view(*reso)
 
 
+def vertex_colours(net, xyz, vd, bs):
+    """util.recon.marching_cubes' colour loop."""
+    rgb = torch.empty(len(xyz), 3, device="cuda")
+    with torch.no_grad():
+        for first in range(0, len(xyz), bs):
+            out = net(xyz[None, first:first + bs], coarse=True, viewdirs=vd[None, first:first + bs])
+            rgb[first:first + bs] = out[0, :, :3]
+    return rgb
+
+
+def attrs_call(vol, iso, c1, c2):
+    """pnr_mc_count on a fresh workspace, then a closure that launches pnr_mc_vertex_attrs on it; -> (closure, n_verts,
+    (xyz, viewdirs))."""
+    import pnr_native as pn
+    L = pn.lib()
+    nx, ny, nz = vol.shape
+    ws = torch.empty(int(L.pnr_mc_workspace_bytes(nx, ny, nz)), dtype=torch.uint8, device="cuda")
+    counts = torch.empty(2, dtype=torch.int64, device="cuda")
+    s = pn.stream_ptr(vol.device)
+    pn.check(L.pnr_mc_count(pn.dptr(vol), nx, ny, nz, iso, C.c_void_p(counts.data_ptr()), C.c_void_p(ws.data_ptr()),
+                            ws.numel(), s))
+    nv = int(counts[0])
+    normals = torch.empty(nv, 3, dtype=torch.float64, device="cuda")
+    xyz, vd = torch.empty(nv, 3, device="cuda"), torch.empty(nv, 3, device="cuda")
+    lo, hi = (C.c_double * 3)(*c1), (C.c_double * 3)(*c2)
+
+    def launch():
+        pn.check(L.pnr_mc_vertex_attrs(pn.dptr(vol), nx, ny, nz, iso, lo, hi, C.c_void_p(normals.data_ptr()),
+                                       pn.dptr(xyz), pn.dptr(vd), nv, C.c_void_p(ws.data_ptr()), ws.numel(), s))
+        return ws                       # keeps the workspace alive with the closure
+    return launch, nv, (xyz, vd)
+
+
 def timed(fn, reps):
     out, ms = None, []
     for _ in range(reps):
@@ -70,6 +108,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--engine", default="tc")
     ap.add_argument("--eval-batch-size", type=int, default=100000)
+    ap.add_argument("--colors", action="store_true", help="also time the vertex attributes and vertex colours")
     a = ap.parse_args()
     import pnr_native as pn
     net = c2_net(a.engine)
@@ -94,6 +133,14 @@ def main():
         res[str(r)] = {"points": n, "sigma_ms": s_med, "sigma_ms_min": s_min, "points_per_s": n / s_med * 1e3,
                        "mc_ms": m_med, "mc_ms_min": m_min, "verts": int(v.shape[0]), "tris": int(t.shape[0]),
                        "mc_workspace_mb": pn.lib().pnr_mc_workspace_bytes(r, r, r) / 2 ** 20}
+        if a.colors:
+            launch, nv, (xyz, vd) = attrs_call(vol, iso, c1, c2)
+            launch()
+            _, a_med, a_min = timed(launch, a.reps)
+            vertex_colours(net, xyz, vd, a.eval_batch_size)
+            _, f_med, f_min = timed(lambda: vertex_colours(net, xyz, vd, a.eval_batch_size), a.reps)
+            res[str(r)].update({"colour_verts": nv, "attrs_ms": a_med, "attrs_ms_min": a_min, "vertex_field_ms": f_med,
+                                "vertex_field_ms_min": f_min, "vertex_points_per_s": nv / f_med * 1e3})
     print(json.dumps(res))
 
 

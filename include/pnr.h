@@ -494,6 +494,62 @@ int pnr_mc_vertex_attrs(const float* vol, int32_t nx, int32_t ny, int32_t nz, do
                         const double* hi, double* normals, float* xyz, float* viewdirs, int64_t n_verts,
                         void* workspace, size_t workspace_bytes, void* stream);
 
+/* Narrow-band marching cubes: the mesh of the entry points above with every cell outside the active blocks treated as
+ * empty and the vertices no remaining triangle uses dropped (the order stays the dense one: vertex ids by (grid
+ * point, axis), triangles by cell, then table order).  Only the blocks the surface crosses, seen on a coarse lattice,
+ * are refined, so sigma is evaluated and workspace taken for the band around the surface instead of the whole grid.
+ * reso: HOST int32[3] as pnr_grid_points takes it; block: b cells per side, 2 <= b <= 256; apron: 0 or 1.
+ *   blocks       block i of an axis covers the cells [i b, min((i + 1) b, n - 1)); nb = ceil((n - 1) / b) per axis.
+ *   lattice      the grid indices min(j b, n - 1), j = 0 .. nb, per axis: (nb0 + 1)(nb1 + 1)(nb2 + 1) grid points in
+ *                ij order, so block i's corners are lattice points i and i + 1.
+ *   seeded       a block whose 8 corners are not all in the same state (inside = finite and sigma > iso);
+ *   active       a block that is seeded or has a seeded one among its 26 neighbours.
+ *   refinement   the grid points of the active blocks' closed cells ([i b, min((i + 1) b, n - 1)] per axis), with
+ *                apron = 1 widened by one point on each side (the neighbours the vertex normals read), in ij order
+ *                (x slowest), as the grid orders them.
+ * Where every non-empty cell of the dense extraction lies in an active block the mesh is the dense one, bit for bit;
+ * otherwise pieces are missing (a feature smaller than a block that no lattice point sees) and the mesh can be open
+ * where the surface leaves the band.
+ *
+ *   pnr_band_plan_bytes     the plan buffer for reso / block / apron (0 when they are invalid); it grows with the
+ *                           block grid (a few bytes per block and per run of points: 2 or 3 runs per block per axis).
+ *   pnr_band_lattice_points lattice points [first, first+count) -> xyz / viewdirs, bit-equal to pnr_grid_points' at
+ *                           the same grid index.
+ *   pnr_band_plan           coarse [nb0 + 1][nb1 + 1][nb2 + 1] fp32 sigma of the lattice -> the plan (active blocks and
+ *                           the offsets that index the refinement set, and a header recording reso, block, apron and
+ *                           the point count); counts_out (int64[2], DEVICE) = active blocks, refinement points.
+ *   pnr_band_points         refinement points [first, first+count) -> xyz / viewdirs, as pnr_band_lattice_points.
+ *                           n_points must be the plan's count; no point past it is written.
+ *   pnr_band_mc_workspace_bytes  the marching-cubes workspace for n_points refinement points (37 bytes per point).
+ *   pnr_band_mc_count / pnr_band_mc_emit / pnr_band_mc_vertex_attrs  pnr_mc_count / pnr_mc_emit /
+ *                           pnr_mc_vertex_attrs over sigma [n_points], the field at the refinement points in their
+ *                           order, with the same plan and workspace on the same stream; the same arithmetic, exclusive
+ *                           scans and no atomics, so repeated calls give the same bits.  Each reads the plan's header
+ *                           back (one synchronise of the stream) and refuses a plan made for another reso / block /
+ *                           apron or another n_points; vertex attributes need apron = 1.
+ * Errors: dimensions < 1 or above 2^36 points, block outside [2, 256], apron not 0 / 1, ranges outside the lattice or
+ * the refinement set, a plan that does not match the call, negative sizes, NULL pointers -> PNR_ERR_INVALID; a plan
+ * buffer below pnr_band_plan_bytes or a workspace below pnr_band_mc_workspace_bytes -> PNR_ERR_WORKSPACE. */
+size_t pnr_band_plan_bytes(const int32_t* reso, int32_t block, int32_t apron);
+int pnr_band_lattice_points(const double* lo, const double* hi, const int32_t* reso, int32_t block, int64_t first,
+                            int64_t count, float* xyz, float* viewdirs, void* stream);
+int pnr_band_plan(const float* coarse, const int32_t* reso, int32_t block, double iso, int32_t apron,
+                  int64_t* counts_out, void* plan, size_t plan_bytes, void* stream);
+int pnr_band_points(const double* lo, const double* hi, const int32_t* reso, int32_t block, int32_t apron,
+                    const void* plan, size_t plan_bytes, int64_t n_points, int64_t first, int64_t count, float* xyz,
+                    float* viewdirs, void* stream);
+size_t pnr_band_mc_workspace_bytes(int64_t n_points);
+int pnr_band_mc_count(const float* sigma, int64_t n_points, const int32_t* reso, int32_t block, int32_t apron,
+                      double iso, const void* plan, size_t plan_bytes, int64_t* counts_out, void* workspace,
+                      size_t workspace_bytes, void* stream);
+int pnr_band_mc_emit(const float* sigma, int64_t n_points, const int32_t* reso, int32_t block, int32_t apron,
+                     double iso, const void* plan, size_t plan_bytes, double* verts, int64_t* tris, int64_t n_verts,
+                     int64_t n_tris, void* workspace, size_t workspace_bytes, void* stream);
+int pnr_band_mc_vertex_attrs(const float* sigma, int64_t n_points, const int32_t* reso, int32_t block, int32_t apron,
+                             double iso, const double* lo, const double* hi, const void* plan, size_t plan_bytes,
+                             double* normals, float* xyz, float* viewdirs, int64_t n_verts, void* workspace,
+                             size_t workspace_bytes, void* stream);
+
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.
  * engine = PNR_ENGINE_SIMT: fp32 FFMA SGEMM; PNR_ENGINE_TC (or AUTO): split-bf16 wgmma GEMM (3 products, fp32

@@ -169,6 +169,20 @@ def declare(L):
         L.pnr_mc_vertex_attrs.argtypes = [vp, i32, i32, i32, f64, P(f64), P(f64), vp, vp, vp, i64, vp, sz, vp]
         for name in ("pnr_grid_points", "pnr_mc_count", "pnr_mc_emit", "pnr_mc_vertex_attrs"):
             getattr(L, name).restype = C.c_int
+        L.pnr_band_plan_bytes.argtypes = [P(i32), i32, i32]
+        L.pnr_band_plan_bytes.restype = sz
+        L.pnr_band_lattice_points.argtypes = [P(f64), P(f64), P(i32), i32, i64, i64, vp, vp, vp]
+        L.pnr_band_plan.argtypes = [vp, P(i32), i32, f64, i32, vp, vp, sz, vp]
+        L.pnr_band_points.argtypes = [P(f64), P(f64), P(i32), i32, i32, vp, sz, i64, i64, i64, vp, vp, vp]
+        L.pnr_band_mc_workspace_bytes.argtypes = [i64]
+        L.pnr_band_mc_workspace_bytes.restype = sz
+        L.pnr_band_mc_count.argtypes = [vp, i64, P(i32), i32, i32, f64, vp, sz, vp, vp, sz, vp]
+        L.pnr_band_mc_emit.argtypes = [vp, i64, P(i32), i32, i32, f64, vp, sz, vp, vp, i64, i64, vp, sz, vp]
+        L.pnr_band_mc_vertex_attrs.argtypes = [vp, i64, P(i32), i32, i32, f64, P(f64), P(f64), vp, sz, vp, vp, vp, i64,
+                                               vp, sz, vp]
+        for name in ("pnr_band_lattice_points", "pnr_band_plan", "pnr_band_points", "pnr_band_mc_count",
+                     "pnr_band_mc_emit", "pnr_band_mc_vertex_attrs"):
+            getattr(L, name).restype = C.c_int
     L.pnr_set_deterministic.argtypes = [C.c_int]
     L.pnr_set_deterministic.restype = C.c_int
     L.pnr_get_deterministic.restype = C.c_int
@@ -354,6 +368,108 @@ def marching_cubes(vol, iso, *, bounds=None):
         check(L.pnr_mc_vertex_attrs(dptr(vol, "vol"), nx, ny, nz, float(iso), (C.c_double * 3)(*map(float, lo)),
                                     (C.c_double * 3)(*map(float, hi)), C.c_void_p(normals.data_ptr()), dptr(xyz),
                                     dptr(viewdirs), nv, C.c_void_p(ws.data_ptr()), ws.numel(), s))
+    return verts, tris, normals, xyz, viewdirs
+
+
+BAND_MAX_BLOCK = 256
+
+
+def _reso3(reso):
+    return (C.c_int32 * 3)(*map(int, reso))
+
+
+def _bounds3(lo, hi):
+    return (C.c_double * 3)(*map(float, lo)), (C.c_double * 3)(*map(float, hi))
+
+
+def band_lattice_size(reso, block):
+    """Points of the narrow band's coarse lattice: the grid indices min(j * block, n - 1), j = 0 .. ceil((n - 1) /
+    block), per axis."""
+    m = [(int(n) - 1 + block - 1) // block + 1 for n in reso]
+    return m[0] * m[1] * m[2]
+
+
+def band_lattice_points(lo, hi, reso, block, first, count, xyz, viewdirs=None):
+    """pnr_band_lattice_points: lattice points [first, first+count) into xyz / viewdirs, as grid_points writes them."""
+    dev = xyz.device
+    with torch.cuda.device(dev):
+        check(lib().pnr_band_lattice_points(*_bounds3(lo, hi), _reso3(reso), int(block), int(first), int(count),
+                                            dptr(xyz, "xyz"), dptr(viewdirs, "viewdirs"), stream_ptr(dev)))
+
+
+class BandPlan:
+    """pnr_band_plan's result: the plan buffer (a CUDA byte tensor) and its counts."""
+
+    def __init__(self, reso, block, apron, buf, n_active, n_points):
+        self.reso, self.block, self.apron, self.buf = reso, block, apron, buf
+        self.n_active, self.n_points = n_active, n_points
+
+    def args(self):
+        return _reso3(self.reso), self.block, int(self.apron)
+
+
+def band_plan(coarse, reso, block, iso, apron=False):
+    """pnr_band_plan on the lattice's fp32 CUDA sigma (band_lattice_size(reso, block) values) -> BandPlan.
+    Synchronises once, to read the active-block and refinement-point counts."""
+    reso, block = [int(r) for r in reso], int(block)
+    dev = coarse.device
+    L = lib()
+    nbytes = int(L.pnr_band_plan_bytes(_reso3(reso), block, int(bool(apron))))
+    if nbytes == 0:
+        raise RuntimeError(f"band_plan: invalid grid {reso} or block {block}")
+    if coarse.numel() != band_lattice_size(reso, block):
+        raise RuntimeError(f"band_plan: coarse sigma has {coarse.numel()} values, the lattice "
+                           f"{band_lattice_size(reso, block)}")
+    buf = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(L.pnr_band_plan(dptr(coarse, "coarse"), _reso3(reso), block, float(iso), int(bool(apron)),
+                              C.c_void_p(counts.data_ptr()), C.c_void_p(buf.data_ptr()), nbytes, stream_ptr(dev)))
+        n_active, n_points = counts.tolist()
+    return BandPlan(reso, block, bool(apron), buf, n_active, n_points)
+
+
+def band_points(plan, lo, hi, first, count, xyz, viewdirs=None):
+    """pnr_band_points: refinement points [first, first+count) of `plan` into xyz / viewdirs."""
+    dev = xyz.device
+    with torch.cuda.device(dev):
+        check(lib().pnr_band_points(*_bounds3(lo, hi), *plan.args(), C.c_void_p(plan.buf.data_ptr()), plan.buf.numel(),
+                                    plan.n_points, int(first), int(count), dptr(xyz, "xyz"),
+                                    dptr(viewdirs, "viewdirs"), stream_ptr(dev)))
+
+
+def band_marching_cubes(sigma, plan, iso, *, bounds=None):
+    """pnr_band_mc_count + pnr_band_mc_emit on the fp32 CUDA sigma of plan's refinement points, in their order ->
+    (vertices float64 [N, 3] in grid index space, triangles int64 [M, 3]), as marching_cubes returns them.
+    Synchronises once, to size the outputs.  With bounds = (lo, hi), pnr_band_mc_vertex_attrs also runs (the plan
+    must have been made with apron) and the result is (vertices, triangles, normals, xyz, viewdirs)."""
+    if sigma.numel() != plan.n_points:
+        raise RuntimeError(f"band_marching_cubes: sigma has {sigma.numel()} values, the plan {plan.n_points} points")
+    if bounds is not None and not plan.apron:
+        raise RuntimeError("band_marching_cubes: vertex attributes need a plan made with apron=True")
+    dev = sigma.device
+    L = lib()
+    M = plan.n_points
+    ws = torch.empty(max(int(L.pnr_band_mc_workspace_bytes(M)), 1), dtype=torch.uint8, device=dev)
+    pp = (C.c_void_p(plan.buf.data_ptr()), plan.buf.numel())
+    head = (dptr(sigma, "sigma"), M, *plan.args(), float(iso))
+    tail = (C.c_void_p(ws.data_ptr()), ws.numel())
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        s = stream_ptr(dev)
+        check(L.pnr_band_mc_count(*head, *pp, C.c_void_p(counts.data_ptr()), *tail, s))
+        nv, nt = counts.tolist()
+        verts = torch.empty(nv, 3, dtype=torch.float64, device=dev)
+        tris = torch.empty(nt, 3, dtype=torch.int64, device=dev)
+        check(L.pnr_band_mc_emit(*head, *pp, C.c_void_p(verts.data_ptr()), C.c_void_p(tris.data_ptr()), nv, nt,
+                                 *tail, s))
+        if bounds is None:
+            return verts, tris
+        normals = torch.empty(nv, 3, dtype=torch.float64, device=dev)
+        xyz = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+        viewdirs = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+        check(L.pnr_band_mc_vertex_attrs(*head, *_bounds3(*bounds), *pp, C.c_void_p(normals.data_ptr()), dptr(xyz),
+                                         dptr(viewdirs), nv, *tail, s))
     return verts, tris, normals, xyz, viewdirs
 
 

@@ -441,6 +441,49 @@ int pnr_mgpu_render_backward_sel(PnrMgpu* h, const PnrShard* shards, const PnrSh
  * j < count.  src: host array of n <= 63 device pointers readable from the current device. */
 int pnr_sum_into(float* dst, const float* const* src, int32_t n, int64_t count, void* stream);
 
+/* Sharded field evaluation for mesh extraction (util/recon.py marching_cubes with several GPUs): the field of ONE object
+ * (scene SB == 1) at points [0, count) of a point set that every device generates itself, channels
+ * [channel, channel + n_channels) of each point's output stored into out0 [count][n_channels] on device 0.
+ * The points are cut into chunks of `chunk` points starting at 0 (the chunks a one-GPU loop of pnr_field_eval calls
+ * evaluates), and shard i takes torch.chunk piece i of the chunk indices: a contiguous run of whole chunks, so every
+ * point is evaluated in the same chunk, at the same offset, as in the one-GPU loop, and the result is bit-equal to it
+ * with every engine.  Shards past the last chunk do nothing.  Per chunk, on device i: the points and view directions
+ * into the shard's workspace (pnr_grid_points / pnr_band_lattice_points / pnr_band_points, or a peer copy of the
+ * chunk's rows of a LIST), one pnr_field_eval, then one small kernel that stores the wanted channels into out0 -- through
+ * peer memory where pnr_mgpu_peer_store(h, i), else into a staging slice of the workspace that is peer-copied to out0.
+ * Shards on the same device run one after another on one stream (as in pnr_mgpu_render); stream0 (device 0) is
+ * ordered after every shard.  Asynchronous, no host synchronisation.
+ * Errors (PNR_ERR_INVALID): an unknown kind, bad reso / block / apron, count outside the grid or lattice, count !=
+ * n_points for BAND, NULL LIST rows or BAND plan, chunk < 1, a channel range outside [0, d_out), a scene with SB != 1;
+ * PNR_ERR_WORKSPACE: a shard workspace below pnr_mgpu_field_workspace_bytes.  Every shard with chunks is checked before
+ * anything is enqueued. */
+enum { PNR_POINTS_GRID = 1, PNR_POINTS_LATTICE = 2, PNR_POINTS_BAND = 3, PNR_POINTS_LIST = 4 };
+
+typedef struct PnrPointSource {   /* which points; host struct                                                           */
+  int32_t kind;                   /* PNR_POINTS_*                                                                        */
+  double lo[3], hi[3];            /* GRID / LATTICE / BAND: the bounds pnr_grid_points / pnr_band_*_points take           */
+  int32_t reso[3];                /* GRID / LATTICE / BAND                                                               */
+  int32_t block, apron;           /* LATTICE (block) / BAND (block, apron): as pnr_band_lattice_points / pnr_band_points */
+  int64_t n_points;               /* BAND: the plan's refinement point count (must equal count)                          */
+  const float* xyz0;              /* LIST: [count][3] points on DEVICE 0                                                 */
+  const float* viewdirs0;         /* LIST: [count][3] view directions on DEVICE 0                                        */
+} PnrPointSource;
+
+typedef struct PnrFieldShard {    /* device i's piece (pointers on device i)                                             */
+  const PnrScene* scene;          /* the scene on device i (shard 0: device 0's own); SB == 1                            */
+  const PnrMlp* mlp;              /* evaluated with scene->proj_coarse, as pnr_field_eval does                           */
+  const void* plan;               /* BAND: the pnr_band_plan buffer on device i                                          */
+  size_t plan_bytes;
+  void* workspace;                /* >= pnr_mgpu_field_workspace_bytes(scene, mlp, chunk, engine)                        */
+  size_t workspace_bytes;
+  void* stream;                   /* stream on device i (NULL: the handle's own; shard 0 always runs on stream0)         */
+} PnrFieldShard;
+
+size_t pnr_mgpu_field_workspace_bytes(const PnrScene* scene, const PnrMlp* mlp, int64_t chunk, int32_t engine);
+int pnr_mgpu_field_eval(PnrMgpu* h, const PnrFieldShard* shards, const PnrPointSource* src, int64_t count,
+                        int64_t chunk, int32_t engine, int32_t channel, int32_t n_channels, float* out0,
+                        void* stream0);
+
 /* ---- mesh extraction: util/recon.py marching_cubes (src/util/recon.py:12-78) ------------------------------------ */
 
 /* The evaluation grid of recon.py:43, util.gen_grid(*zip(lo, hi, reso), ij_indexing=True) (src/util/util.py:93-110):

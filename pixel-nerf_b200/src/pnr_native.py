@@ -81,6 +81,20 @@ class PnrShardCam(C.Structure):
     _fields_ = [("cam", PnrCameraGrad), ("d_rays", _fp)]
 
 
+POINTS_GRID, POINTS_LATTICE, POINTS_BAND, POINTS_LIST = 1, 2, 3, 4
+
+
+class PnrPointSource(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("lo", C.c_double * 3), ("hi", C.c_double * 3), ("reso", C.c_int32 * 3),
+                ("block", C.c_int32), ("apron", C.c_int32), ("n_points", C.c_int64), ("xyz0", _fp),
+                ("viewdirs0", _fp)]
+
+
+class PnrFieldShard(C.Structure):
+    _fields_ = [("scene", C.POINTER(PnrScene)), ("mlp", C.POINTER(PnrMlp)), ("plan", _fp), ("plan_bytes", C.c_size_t),
+                ("workspace", _fp), ("workspace_bytes", C.c_size_t), ("stream", _fp)]
+
+
 _lib = None
 
 
@@ -159,6 +173,11 @@ def declare(L):
                      "pnr_mgpu_render_backward", "pnr_mgpu_render_backward_cam", "pnr_mgpu_render_backward_sel",
                      "pnr_sum_into"):
             getattr(L, name).restype = C.c_int
+    if hasattr(L, "pnr_mgpu_field_eval"):  # (the host-emulator builds of tests/cuda_emu have it only with mesh extraction)
+        L.pnr_mgpu_field_workspace_bytes.argtypes = [P(PnrScene), P(PnrMlp), i64, i32]
+        L.pnr_mgpu_field_workspace_bytes.restype = sz
+        L.pnr_mgpu_field_eval.argtypes = [vp, P(PnrFieldShard), P(PnrPointSource), i64, i64, i32, i32, i32, vp, vp]
+        L.pnr_mgpu_field_eval.restype = C.c_int
     if hasattr(L, "pnr_grid_points"):     # (the host-emulator build of tests/cuda_emu has no mesh extraction)
         f64 = C.c_double
         L.pnr_grid_points.argtypes = [P(f64), P(f64), P(i32), i64, i64, vp, vp, vp]
@@ -471,6 +490,29 @@ def band_marching_cubes(sigma, plan, iso, *, bounds=None):
         check(L.pnr_band_mc_vertex_attrs(*head, *_bounds3(*bounds), *pp, C.c_void_p(normals.data_ptr()), dptr(xyz),
                                          dptr(viewdirs), nv, *tail, s))
     return verts, tris, normals, xyz, viewdirs
+
+
+def point_source(kind, lo=(0.0, 0.0, 0.0), hi=(0.0, 0.0, 0.0), reso=(1, 1, 1), block=0, apron=False, n_points=0,
+                 xyz0=None, viewdirs0=None):
+    """PnrPointSource for pnr_mgpu_field_eval: POINTS_GRID (lo, hi, reso), POINTS_LATTICE (+ block), POINTS_BAND
+    (+ apron and the plan's n_points) or POINTS_LIST (xyz0 / viewdirs0 [count, 3] fp32 CUDA tensors on gpus[0])."""
+    s = PnrPointSource()
+    s.kind = int(kind)
+    s.lo[:], s.hi[:], s.reso[:] = [float(v) for v in lo], [float(v) for v in hi], [int(r) for r in reso]
+    s.block, s.apron, s.n_points = int(block), int(bool(apron)), int(n_points)
+    s.xyz0, s.viewdirs0 = dptr(xyz0, "xyz0"), dptr(viewdirs0, "viewdirs0")
+    return s
+
+
+def mgpu_field_eval(handle, shards, src, count, chunk, engine, channel, out0):
+    """pnr_mgpu_field_eval: channels [channel, channel + out0.shape[1]) of the field at the source's points [0, count),
+    in chunks of `chunk` points sharded over the handle's devices -> out0 [count, n_channels] (fp32 CUDA, gpus[0]),
+    ordered on out0's device's current stream.  shards: a PnrFieldShard array, one per device of the handle."""
+    dev = out0.device
+    with torch.cuda.device(dev):
+        check(lib().pnr_mgpu_field_eval(handle, shards, C.byref(src), int(count), int(chunk), int(engine), int(channel),
+                                        int(out0.shape[1]), dptr(out0, "out0"), stream_ptr(dev)))
+    return out0
 
 
 def profile_begin():

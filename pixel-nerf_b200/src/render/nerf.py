@@ -93,6 +93,24 @@ class _RenderWrapper(torch.nn.Module):
         return _wrapper_output(self.renderer, outputs, self.simple_output)
 
 
+def broadcast_to(gpus, t, dev, handle):
+    """A copy on `dev` of the buffer `t` on gpus[0], through pnr_mgpu_broadcast on the handle `handle()` of `gpus`
+    (peer copy over NVLink, enqueued on torch's current streams so the caching allocator's stream ordering holds)."""
+    import ctypes as C
+    n = len(gpus)
+    t = t.contiguous()
+    with torch.cuda.device(dev):
+        dst = torch.empty_like(t, device=dev)
+    ptrs, streams = (C.c_void_p * n)(), (C.c_void_p * n)()
+    for i, g in enumerate(gpus):
+        streams[i] = torch.cuda.current_stream(torch.device("cuda", g)).cuda_stream
+        if g == dev.index:
+            ptrs[i] = dst.data_ptr()
+    pn.check(pn.lib().pnr_mgpu_broadcast(handle(), C.c_void_p(t.data_ptr()), ptrs, t.numel() * t.element_size(),
+                                         streams))
+    return dst
+
+
 class _SceneReplica:
     """Everything the fused render path reads, on ANOTHER GPU of the same process: channels-last latent, cameras, fp32
     weights, packed tensor-engine weights and projected maps.  Filled by peer copies (NVLink) of the primary device's
@@ -186,21 +204,8 @@ class _ShardedRender(torch.nn.Module):
         return self._handle
 
     def _send(self, t, dev):
-        """One buffer of the primary device to `dev` through pnr_mgpu_broadcast (peer copy over NVLink, enqueued on
-        torch's current streams so the caching allocator's stream ordering holds)."""
-        import ctypes as C
-        n = len(self.gpus)
-        t = t.contiguous()
-        with torch.cuda.device(dev):
-            dst = torch.empty_like(t, device=dev)
-        ptrs, streams = (C.c_void_p * n)(), (C.c_void_p * n)()
-        for i, g in enumerate(self.gpus):
-            streams[i] = torch.cuda.current_stream(torch.device("cuda", g)).cuda_stream
-            if g == dev.index:
-                ptrs[i] = dst.data_ptr()
-        pn.check(pn.lib().pnr_mgpu_broadcast(self._mgpu(), C.c_void_p(t.data_ptr()), ptrs, t.numel() * t.element_size(),
-                                             streams))
-        return dst
+        """One buffer of the primary device to `dev` through pnr_mgpu_broadcast (see `broadcast_to`)."""
+        return broadcast_to(self.gpus, t, dev, self._mgpu)
 
     def __del__(self):
         try:

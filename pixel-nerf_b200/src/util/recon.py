@@ -5,7 +5,8 @@ Mesh reconstruction tools (the reference's src/util/recon.py), on the GPU.
 library's own marching cubes (`pnr_grid_points`, `pnr_field_eval`, `pnr_mc_count` / `pnr_mc_emit`, include/pnr.h):
 the grid, the sigma volume and the mesh stay on the device, and only the mesh comes back.  With `return_colors`,
 `pnr_mc_vertex_attrs` adds normals and the field colours each vertex.  With `block`, sigma is evaluated on a coarse
-lattice first and only the blocks the surface crosses are refined and meshed (`pnr_band_*`).  There is no CPU path.
+lattice first and only the blocks the surface crosses are refined and meshed (`pnr_band_*`).  With `gpus`, every field
+pass is sharded over several GPUs (`pnr_mgpu_field_eval`) and the rest stays on the first.  There is no CPU path.
 """
 import warnings
 
@@ -27,6 +28,7 @@ def marching_cubes(
     device=None,
     return_colors=False,
     block=None,
+    gpus=None,
 ):
     """
     Run marching cubes on network.
@@ -56,6 +58,12 @@ def marching_cubes(
     remaining triangle uses dropped; where every cell the surface crosses lies in such a block it is the dense result,
     bit for bit.  A feature smaller than a block that no lattice point sees is missed, and the mesh can be open where
     the surface leaves the band.
+    :param gpus None (default) or one device: everything on `device`.  A list of CUDA device indices [g0, g1, ...]
+    with g0 the extraction device (`device`, or occu_net's): every field evaluation -- the sigma grid, the band's
+    lattice and refinement points, the vertex colours -- is cut into the same eval_batch_size chunks as on one GPU and
+    the chunks are shared out among the devices in contiguous runs; gpus[i] evaluates its run from a copy of the
+    scene and weights and sends the values to g0.  A device may repeat ([0, 0]: two shards on one card).  Marching
+    cubes, the band plan and the vertex attributes stay on g0.  The result is bit-equal to the call without gpus.
     """
     if occu_net.use_viewdirs:
         warnings.warn(
@@ -74,18 +82,25 @@ def marching_cubes(
         if isinstance(block, bool) or not isinstance(block, (int, np.integer)) or not 2 <= block <= pn.BAND_MAX_BLOCK:
             raise ValueError(f"block must be None or an int in [2, {pn.BAND_MAX_BLOCK}], got {block!r}")
         block = int(block)
+    if gpus is not None:
+        gpus = [int(g) for g in gpus]
+        if not gpus or gpus[0] != (device.index if device.index is not None else torch.cuda.current_device()):
+            raise ValueError(f"gpus[0] must be the extraction device {device}, got gpus = {gpus}")
     is_train = occu_net.training
     occu_net.eval()
+    field = None
     try:
         with torch.no_grad():
+            if gpus is not None and len(gpus) > 1:
+                field = _ShardedField(occu_net, gpus, coarse)
             if block is not None:
                 vertices, triangles, *colors = _band(occu_net, c1, c2, reso, isosurface, sigma_idx, eval_batch_size,
-                                                     coarse, device, return_colors, block)
+                                                     coarse, device, return_colors, block, field)
                 return _scaled(vertices, triangles, c1, c2, reso, *colors)
             print("Evaluating sigma @", N, "points")
             bs = max(1, min(int(eval_batch_size), N))
             sigmas = _sigma(occu_net, N, bs, lambda f, n, p, d: pn.grid_points(c1, c2, reso, f, n, p, d), coarse,
-                            sigma_idx, device)
+                            sigma_idx, device, field, pn.point_source(pn.POINTS_GRID, c1, c2, reso))
 
             print("Running marching cubes")
             if not return_colors:
@@ -96,10 +111,12 @@ def marching_cubes(
                 vertices, triangles, normals, xyz, vd = pn.marching_cubes(sigmas.view(*reso), isosurface,
                                                                           bounds=(c1, c2))
                 print("Evaluating colour @", len(xyz), "vertices")
-                rgb = _colours(occu_net, xyz, vd, bs, coarse, device)
+                rgb = _colours(occu_net, xyz, vd, bs, coarse, device, field)
                 normals, rgb = normals.cpu().numpy(), rgb.cpu().numpy()
             vertices, triangles = vertices.cpu().numpy(), triangles.cpu().numpy()
     finally:
+        if field is not None:
+            field.close()
         if is_train:
             occu_net.train()
     if return_colors:
@@ -114,8 +131,11 @@ def _scaled(vertices, triangles, c1, c2, reso, *colors):
     return (vertices + c1, triangles) + colors
 
 
-def _sigma(occu_net, count, bs, points, coarse, sigma_idx, device):
-    """sigma [count] of the points `points(first, n, xyz, viewdirs)` writes, in bs chunks"""
+def _sigma(occu_net, count, bs, points, coarse, sigma_idx, device, field=None, src=None):
+    """sigma [count] of the points `points(first, n, xyz, viewdirs)` writes, in bs chunks (with `field`, a
+    _ShardedField: the same points, as the PnrPointSource `src` describes them, over its GPUs)"""
+    if field is not None:
+        return field.eval(src, count, bs, sigma_idx, 1).view(-1)
     pts = torch.empty(bs, 3, dtype=torch.float32, device=device)
     vd = torch.empty(bs, 3, dtype=torch.float32, device=device)
     sigmas = torch.empty(count, dtype=torch.float32, device=device)
@@ -127,7 +147,9 @@ def _sigma(occu_net, count, bs, points, coarse, sigma_idx, device):
     return sigmas
 
 
-def _colours(occu_net, xyz, vd, bs, coarse, device):
+def _colours(occu_net, xyz, vd, bs, coarse, device, field=None):
+    if field is not None:
+        return field.eval(pn.point_source(pn.POINTS_LIST, xyz0=xyz, viewdirs0=vd), len(xyz), bs, 0, 3)
     rgb = torch.empty(len(xyz), 3, dtype=torch.float32, device=device)
     for first in range(0, len(xyz), bs):
         out = occu_net(xyz[None, first:first + bs], coarse=coarse, viewdirs=vd[None, first:first + bs])
@@ -135,29 +157,105 @@ def _colours(occu_net, xyz, vd, bs, coarse, device):
     return rgb
 
 
-def _band(occu_net, c1, c2, reso, isosurface, sigma_idx, eval_batch_size, coarse, device, return_colors, block):
+def _band(occu_net, c1, c2, reso, isosurface, sigma_idx, eval_batch_size, coarse, device, return_colors, block,
+          field=None):
     """The narrow-band path of marching_cubes -> numpy (vertices in grid index units, triangles[, normals, rgb]).
     Nothing on it is sized by the full grid."""
     n_lat = pn.band_lattice_size(reso, block)
     print("Evaluating sigma @", n_lat, "coarse lattice points")
     bs = max(1, min(int(eval_batch_size), n_lat))
     lattice = _sigma(occu_net, n_lat, bs, lambda f, n, p, d: pn.band_lattice_points(c1, c2, reso, block, f, n, p, d),
-                     coarse, sigma_idx, device)
+                     coarse, sigma_idx, device, field, pn.point_source(pn.POINTS_LATTICE, c1, c2, reso, block))
     plan = pn.band_plan(lattice, reso, block, isosurface, apron=return_colors)
     del lattice
     M = plan.n_points
     print("Evaluating sigma @", M, "points in", plan.n_active, "active blocks")
     bs = max(1, min(int(eval_batch_size), max(M, 1)))
+    if field is not None:
+        field.set_plan(plan)
     sigmas = _sigma(occu_net, M, bs, lambda f, n, p, d: pn.band_points(plan, c1, c2, f, n, p, d), coarse, sigma_idx,
-                    device)
+                    device, field, pn.point_source(pn.POINTS_BAND, c1, c2, reso, block, plan.apron, M))
     print("Running marching cubes")
     if not return_colors:
         return tuple(t.cpu().numpy() for t in pn.band_marching_cubes(sigmas, plan, isosurface))
     vertices, triangles, normals, xyz, vd = pn.band_marching_cubes(sigmas, plan, isosurface, bounds=(c1, c2))
     print("Evaluating colour @", len(xyz), "vertices")
     bs = max(1, min(int(eval_batch_size), reso[0] * reso[1] * reso[2]))      # the dense path's chunks
-    rgb = _colours(occu_net, xyz, vd, bs, coarse, device)
+    rgb = _colours(occu_net, xyz, vd, bs, coarse, device, field)
     return tuple(t.cpu().numpy() for t in (vertices, triangles, normals, rgb))
+
+
+class _ShardedField:
+    """occu_net's field over several GPUs for one marching_cubes call: a pnr_mgpu handle over `gpus`, a
+    render.nerf._SceneReplica of the scene and weights for the shards after the first (peer copies through
+    pnr_mgpu_broadcast; one per device, gpus[0] included when it repeats, as bind_parallel does), and
+    pnr_mgpu_field_eval for every field pass.  `close()` destroys the handle and drops the replicas."""
+
+    def __init__(self, occu_net, gpus, coarse):
+        import ctypes as C
+        from render.nerf import _SceneReplica, broadcast_to
+        self.gpus = gpus
+        self.engine = pn.ENGINES[occu_net.engine]
+        use_fine = (not coarse) and occu_net.mlp_fine is not None
+        self.handle = C.c_void_p()
+        pn.check(pn.lib().pnr_mgpu_create((C.c_int32 * len(gpus))(*gpus), len(gpus), C.byref(self.handle)))
+        send = lambda t, d: broadcast_to(gpus, t, d, lambda: self.handle)    # noqa: E731
+        try:
+            self.replicas = {}
+            self.shards = (pn.PnrFieldShard * len(gpus))()
+            self.keep = []
+            for i, g in enumerate(gpus):
+                dev = torch.device("cuda", g)
+                if i == 0:
+                    model = occu_net
+                else:
+                    model = self.replicas.get(g)
+                    if model is None:
+                        model = self.replicas[g] = _SceneReplica(dev)
+                        model.refresh(occu_net, use_fine, send=send)
+                with torch.cuda.device(dev):
+                    scene, mc, mf, keep = model._scene_struct(want_fine=use_fine)
+                mlp = mf if use_fine else mc
+                if use_fine:
+                    scene.proj_coarse = scene.proj_fine      # pnr_field_eval reads proj_coarse for its mlp
+                sh = self.shards[i]
+                sh.scene, sh.mlp = C.pointer(scene), C.pointer(mlp)
+                sh.stream = pn.stream_ptr(dev)
+                self.keep += [scene, mlp, keep]
+        except BaseException:
+            self.close()
+            raise
+
+    def set_plan(self, plan):
+        """The band plan on every device: the buffer itself on gpus[0]'s, a peer copy elsewhere."""
+        from render.nerf import broadcast_to
+        bufs = {self.gpus[0]: plan.buf}
+        for i, g in enumerate(self.gpus):
+            if g not in bufs:
+                bufs[g] = broadcast_to(self.gpus, plan.buf, torch.device("cuda", g), lambda: self.handle)
+            self.shards[i].plan, self.shards[i].plan_bytes = bufs[g].data_ptr(), bufs[g].numel()
+        self.keep.append(bufs)
+
+    def eval(self, src, count, chunk, channel, n_channels):
+        """-> [count, n_channels] fp32 on gpus[0]: channels [channel, channel + n_channels) of the field at the points
+        [0, count) of the PnrPointSource src, in chunks of `chunk` points"""
+        dev0 = torch.device("cuda", self.gpus[0])
+        channel = range(4)[channel]                      # (a negative index counts from the end, as in out[..., idx])
+        need = {}                                        # the shards of a device run in turn: they share one workspace
+        for i, g in enumerate(self.gpus):
+            sh = self.shards[i]
+            need[g] = max(need.get(g, 0), pn.lib().pnr_mgpu_field_workspace_bytes(sh.scene, sh.mlp, chunk, self.engine))
+        ws = {g: pn.workspace(torch.device("cuda", g), n) for g, n in need.items()}
+        for i, g in enumerate(self.gpus):
+            self.shards[i].workspace, self.shards[i].workspace_bytes = ws[g].data_ptr(), ws[g].numel()
+        out = torch.empty(count, n_channels, dtype=torch.float32, device=dev0)
+        return pn.mgpu_field_eval(self.handle, self.shards, src, count, chunk, self.engine, channel, out)
+
+    def close(self):
+        if self.handle:
+            pn.check(pn.lib().pnr_mgpu_destroy(self.handle))
+            self.handle = None
+        self.replicas, self.keep = {}, []
 
 
 def save_obj(vertices, triangles, path, vert_rgb=None, vert_normals=None):

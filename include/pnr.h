@@ -593,6 +593,30 @@ int pnr_band_mc_vertex_attrs(const float* sigma, int64_t n_points, const int32_t
                              double* normals, float* xyz, float* viewdirs, int64_t n_verts, void* workspace,
                              size_t workspace_bytes, void* stream);
 
+/* TSDF fusion of rendered depth maps (no counterpart in the reference; util/recon.py fuse_views): a truncated signed
+ * distance volume tsdf [nx][ny][nz] fp32 (DEVICE) from V views' depth and opacity maps depth / opacity [V][H][W] fp32
+ * (DEVICE: the renderer's depth sum(w z) and weights.sum(-1) of each pixel, the pixel order of pnr_gen_rays) and their
+ * camera-to-world poses_c2w [V][4][4] fp32 (DEVICE, as pnr_gen_rays takes them).  fx, fy, cx, cy: HOST floats, as
+ * pnr_gen_rays; lo, hi (double[3]) and reso (int32[3]): HOST, as pnr_grid_points.  One thread per voxel, the views in
+ * order, no atomics: repeated calls give the same bits.  All in float64 with round-to-nearest intrinsics.  Voxel x is
+ * pnr_grid_points' point (lo + i (hi - lo) / (n - 1) rounded to fp32).  Per view v, with R = pose[:3, :3], t =
+ * pose[:3, 3]:
+ *   q = R^T (x - t), each component (R0j d0 + R1j d1) + R2j d2.  q_z >= 0: v does not see the voxel.
+ *   px = cx + fx q_x / (-q_z), py = cy + fy q_y / q_z (the inverse of pnr_gen_rays: -z forward, +y up, pixel centres on
+ *   integers), rounded to the nearest pixel as floor(p + 0.5) (ties round up).  Outside [0, W-1] x [0, H-1]: v does
+ *   not see the voxel.
+ *   a = opacity of that pixel.  a < min_opacity (or NaN): the pixel saw background, s = +1 (free space).  Otherwise
+ *   s = (depth / a - d) / trunc with d = sqrt((q_x^2 + q_y^2) + q_z^2) (the rays are unit-norm, so depth is a distance
+ *   along the ray); s < -1 (or NaN): occluded, no observation; else s = min(s, 1).
+ * tsdf = the mean of the observations' s (summed in view order).  A voxel with no observation gets -1 (inside) when some
+ * view saw it in front of the camera and inside its image, and +1 (outside) when none did, so every voxel has a value
+ * and pnr_mc_count / pnr_mc_emit mesh -tsdf at iso 0 (positive inside) as they are.
+ * Errors (before any CUDA call): NULL pointers, V, W or H < 1, reso outside [1, 2^36 points], trunc not positive and
+ * finite, min_opacity outside (0, 1] -> PNR_ERR_INVALID. */
+int pnr_tsdf_fuse(const float* depth, const float* opacity, int32_t V, int32_t W, int32_t H, const float* poses_c2w,
+                  float fx, float fy, float cx, float cy, const double* lo, const double* hi, const int32_t* reso,
+                  double trunc, double min_opacity, float* tsdf, void* stream);
+
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.
  * engine = PNR_ENGINE_SIMT: fp32 FFMA SGEMM; PNR_ENGINE_TC (or AUTO): split-bf16 wgmma GEMM (3 products, fp32

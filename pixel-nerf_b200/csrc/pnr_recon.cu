@@ -819,6 +819,51 @@ static int band_mc_setup(const int32_t* reso, int32_t block, int32_t apron, cons
 
 static unsigned grid_for(int64_t n) { return (unsigned)((n + kPtThreads - 1) / kPtThreads); }
 
+// ---- TSDF fusion ---------------------------------------------------------------------------------------------------
+// One thread per voxel (pnr_grid_points' point, in float64), the views in order, the rule of include/pnr.h
+// pnr_tsdf_fuse.  Every operation is one float64 round-to-nearest step, so oracle/pnr_recon_fuse.py gets the same bits.
+__global__ void k_tsdf_fuse(const float* __restrict__ depth, const float* __restrict__ opacity, int V, int W, int H,
+                            const float* __restrict__ poses, double fx, double fy, double cx, double cy, double lo0,
+                            double lo1, double lo2, double hi0, double hi1, double hi2, int nx, int ny, int nz,
+                            double trunc, double min_opacity, float* __restrict__ tsdf) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= (int64_t)nx * ny * nz) return;
+  const int iz = (int)(p % nz);
+  const int iy = (int)((p / nz) % ny);
+  const int ix = (int)(p / ((int64_t)ny * nz));
+  const double x[3] = {(double)linspace_f32(lo0, hi0, nx, ix), (double)linspace_f32(lo1, hi1, ny, iy),
+                       (double)linspace_f32(lo2, hi2, nz, iz)};
+  double sum = 0.0;
+  int n = 0;
+  bool seen = false;
+  for (int v = 0; v < V; ++v) {
+    const float* P = poses + (int64_t)v * 16;          // camera-to-world, row-major 4x4: R = P[:3, :3], t = P[:3, 3]
+    const double d[3] = {__dsub_rn(x[0], (double)P[3]), __dsub_rn(x[1], (double)P[7]), __dsub_rn(x[2], (double)P[11])};
+    double q[3];                                       // R^T (x - t)
+    for (int j = 0; j < 3; ++j)
+      q[j] = __dadd_rn(__dadd_rn(__dmul_rn((double)P[j], d[0]), __dmul_rn((double)P[4 + j], d[1])),
+                       __dmul_rn((double)P[8 + j], d[2]));
+    if (!(q[2] < 0.0)) continue;                       // behind the camera (or on its plane)
+    const double px = __dadd_rn(cx, __ddiv_rn(__dmul_rn(fx, q[0]), -q[2]));
+    const double py = __dadd_rn(cy, __ddiv_rn(__dmul_rn(fy, q[1]), q[2]));
+    const double rx = floor(__dadd_rn(px, 0.5)), ry = floor(__dadd_rn(py, 0.5));    // ties round up
+    if (!(rx >= 0.0 && rx <= (double)(W - 1) && ry >= 0.0 && ry <= (double)(H - 1))) continue;
+    seen = true;
+    const int64_t pix = ((int64_t)v * H + (int)ry) * W + (int)rx;
+    const double a = (double)opacity[pix];
+    double s = 1.0;                                    // background: free space
+    if (a >= min_opacity) {
+      const double dist = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(q[0], q[0]), __dmul_rn(q[1], q[1])), __dmul_rn(q[2], q[2])));
+      s = __ddiv_rn(__dsub_rn(__ddiv_rn((double)depth[pix], a), dist), trunc);
+      if (!(s >= -1.0)) continue;                      // occluded (or NaN): no observation
+      if (s > 1.0) s = 1.0;
+    }
+    sum = __dadd_rn(sum, s);
+    ++n;
+  }
+  tsdf[p] = n > 0 ? __double2float_rn(__ddiv_rn(sum, (double)n)) : (seen ? -1.0f : 1.0f);
+}
+
 }  // namespace pnr
 
 using namespace pnr;
@@ -1086,6 +1131,24 @@ int pnr_band_mc_vertex_attrs(const float* sigma, int64_t n_points, const int32_t
   k_band_vertex_attrs<<<grid_for(n_points), kPtThreads, 0, s>>>(sigma, n_points, g, p, iso, lo[0], lo[1], lo[2], hi[0],
                                                                  hi[1], hi[2], w.flags, w.vid, n_verts, normals, xyz,
                                                                  viewdirs);
+  PNR_LAUNCH_CHECK();
+  return PNR_OK;
+}
+
+int pnr_tsdf_fuse(const float* depth, const float* opacity, int32_t V, int32_t W, int32_t H, const float* poses_c2w,
+                  float fx, float fy, float cx, float cy, const double* lo, const double* hi, const int32_t* reso,
+                  double trunc, double min_opacity, float* tsdf, void* stream) {
+  PNR_CHECK_ARG(depth && opacity && poses_c2w && tsdf, "NULL pointer");
+  PNR_CHECK_ARG(lo && hi && reso, "NULL bounds");
+  PNR_CHECK_ARG(V >= 1 && W >= 1 && H >= 1, "V, W and H must be >= 1");
+  const int rc = check_dims(reso[0], reso[1], reso[2]);
+  if (rc) return rc;
+  PNR_CHECK_ARG(trunc > 0.0 && trunc <= 1.7976931348623157e308, "trunc must be positive and finite");
+  PNR_CHECK_ARG(min_opacity > 0.0 && min_opacity <= 1.0, "min_opacity must be in (0, 1]");
+  const int64_t N = (int64_t)reso[0] * reso[1] * reso[2];
+  k_tsdf_fuse<<<grid_for(N), kPtThreads, 0, (cudaStream_t)stream>>>(
+      depth, opacity, V, W, H, poses_c2w, (double)fx, (double)fy, (double)cx, (double)cy, lo[0], lo[1], lo[2], hi[0],
+      hi[1], hi[2], reso[0], reso[1], reso[2], trunc, min_opacity, tsdf);
   PNR_LAUNCH_CHECK();
   return PNR_OK;
 }

@@ -199,8 +199,10 @@ def declare(L):
         L.pnr_band_mc_emit.argtypes = [vp, i64, P(i32), i32, i32, f64, vp, sz, vp, vp, i64, i64, vp, sz, vp]
         L.pnr_band_mc_vertex_attrs.argtypes = [vp, i64, P(i32), i32, i32, f64, P(f64), P(f64), vp, sz, vp, vp, vp, i64,
                                                vp, sz, vp]
+        L.pnr_tsdf_fuse.argtypes = [vp, vp, i32, i32, i32, vp, f32, f32, f32, f32, P(f64), P(f64), P(i32), f64, f64,
+                                    vp, vp]
         for name in ("pnr_band_lattice_points", "pnr_band_plan", "pnr_band_points", "pnr_band_mc_count",
-                     "pnr_band_mc_emit", "pnr_band_mc_vertex_attrs"):
+                     "pnr_band_mc_emit", "pnr_band_mc_vertex_attrs", "pnr_tsdf_fuse"):
             getattr(L, name).restype = C.c_int
     L.pnr_set_deterministic.argtypes = [C.c_int]
     L.pnr_set_deterministic.restype = C.c_int
@@ -388,6 +390,28 @@ def marching_cubes(vol, iso, *, bounds=None):
                                     (C.c_double * 3)(*map(float, hi)), C.c_void_p(normals.data_ptr()), dptr(xyz),
                                     dptr(viewdirs), nv, C.c_void_p(ws.data_ptr()), ws.numel(), s))
     return verts, tris, normals, xyz, viewdirs
+
+
+def tsdf_fuse(depth, opacity, poses, fx, fy, cx, cy, lo, hi, reso, trunc, min_opacity):
+    """pnr_tsdf_fuse: depth and opacity maps [V, H, W] and camera-to-world poses [V, 4, 4] (fp32 CUDA tensors on one
+    device) -> the fused TSDF [nx, ny, nz] fp32 on that device, positive outside (rule: include/pnr.h)."""
+    if depth.dim() != 3 or opacity.shape != depth.shape:
+        raise RuntimeError(f"tsdf_fuse: depth and opacity must both be [V, H, W], got {tuple(depth.shape)} and "
+                           f"{tuple(opacity.shape)}")
+    V, H, W = depth.shape
+    if tuple(poses.shape) != (V, 4, 4):
+        raise RuntimeError(f"tsdf_fuse: poses must be [{V}, 4, 4], got {tuple(poses.shape)}")
+    dev = depth.device
+    if opacity.device != dev or poses.device != dev:
+        raise RuntimeError(f"tsdf_fuse: depth, opacity and poses must be on one device, got {dev}, {opacity.device} "
+                           f"and {poses.device}")
+    reso = [int(r) for r in reso]
+    tsdf = torch.empty(*reso, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(lib().pnr_tsdf_fuse(dptr(depth, "depth"), dptr(opacity, "opacity"), V, W, H, dptr(poses, "poses"),
+                                  float(fx), float(fy), float(cx), float(cy), *_bounds3(lo, hi), _reso3(reso),
+                                  float(trunc), float(min_opacity), dptr(tsdf), stream_ptr(dev)))
+    return tsdf
 
 
 BAND_MAX_BLOCK = 256

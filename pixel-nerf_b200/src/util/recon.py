@@ -7,6 +7,9 @@ the grid, the sigma volume and the mesh stay on the device, and only the mesh co
 `pnr_mc_vertex_attrs` adds normals and the field colours each vertex.  With `block`, sigma is evaluated on a coarse
 lattice first and only the blocks the surface crosses are refined and meshed (`pnr_band_*`).  With `gpus`, every field
 pass is sharded over several GPUs (`pnr_mgpu_field_eval`) and the rest stays on the first.  There is no CPU path.
+
+`fuse_views` meshes what the renderer shows instead: it renders depth and opacity maps from camera poses, fuses them
+into a TSDF (`pnr_tsdf_fuse`) and meshes that with the same marching cubes.
 """
 import warnings
 
@@ -122,6 +125,123 @@ def marching_cubes(
     if return_colors:
         return _scaled(vertices, triangles, c1, c2, reso, normals, rgb)
     return _scaled(vertices, triangles, c1, c2, reso)
+
+
+def fuse_views(
+    net,
+    renderer,
+    poses,
+    width,
+    height,
+    focal,
+    z_near,
+    z_far,
+    c=None,
+    c1=[-1, -1, -1],
+    c2=[1, 1, 1],
+    reso=[128, 128, 128],
+    trunc=None,
+    min_opacity=0.5,
+    ray_batch_size=50000,
+    gpus=None,
+    return_colors=False,
+):
+    """
+    Mesh the surface the renderer shows: render depth and opacity maps of every view, fuse them into a truncated
+    signed distance field (TSDF) on the grid of marching_cubes, and run marching cubes on it.  Unlike the sigma grid
+    of marching_cubes, every depth sample comes from a real camera with real view directions, so the mesh follows the
+    renders of a model whose sigma depends on the view direction.
+    :param net main NeRF type network, encoded with one object (num_objs == 1), on a CUDA device
+    :param renderer NeRFRenderer; every pixel of every view is rendered through renderer.bind_parallel(net, gpus)
+    with want_weights=True, in ray_batch_size batches in the pixel order of render.render_frames, and the fine pass's
+    depth and weights.sum(-1) (the coarse pass's when renderer.using_fine is off) are kept per pixel
+    :param poses (V, 4, 4) camera-to-world poses, V >= 1 (util.pose_spherical makes a turntable)
+    :param width, height, focal, z_near, z_far, c: the cameras, as util.gen_rays takes them
+    :param c1, c2, reso: the TSDF grid, as marching_cubes takes them (pnr_grid_points' points), each reso >= 2
+    :param trunc truncation distance (world units); default 3 voxel diagonals of the coarsest axis
+    :param min_opacity a pixel of lower opacity saw background, which carves the voxels it sees
+    :param gpus None or a list of CUDA device indices with gpus[0] net's device: the rendering is sharded over them
+    (bind_parallel); fusion, marching cubes and colours run on gpus[0]
+    :param return_colors also return per-vertex normals and colours
+    :return vertices (N, 3) float64 numpy in world coordinates at their true positions, lo + v (hi - lo) / (n - 1)
+    for index coordinate v (unlike marching_cubes, which keeps the reference's (c2 - c1) / reso scale); triangles
+    (M, 3) int64 numpy, counter-clockwise seen from outside.  With return_colors, also normals (N, 3) float64 numpy,
+    unit, outward (pnr_mc_vertex_attrs on the fused volume), and rgb (N, 3) float32 numpy: channels 0-2 of net at the
+    vertex, seen head-on from outside, from the network of the kept pass.  The fusion rule is pnr_tsdf_fuse's
+    (include/pnr.h): the renderer's depth is sum(w z), so the surface distance of a pixel is depth / opacity.
+
+    Example, a turntable at 30 degrees elevation around an object at the origin::
+
+        poses = torch.stack([util.pose_spherical(a, -30.0, 1.3) for a in np.linspace(-180, 180, 65)[:-1]]).cuda()
+        verts, tris = util.recon.fuse_views(net, renderer, poses, 128, 128, focal, 0.8, 1.8, reso=[256] * 3)
+    """
+    from util.util import _intrinsics
+    device = next(net.parameters()).device
+    if device.type != "cuda":
+        raise RuntimeError(f"fuse_views runs on CUDA only (no CPU fallback); got device {device}")
+    if net.num_objs != 1:
+        raise RuntimeError(f"fuse_views needs a network encoded with one object, got num_objs = {net.num_objs}")
+    if gpus is not None:
+        gpus = [int(g) for g in gpus]
+        if not gpus or gpus[0] != (device.index if device.index is not None else torch.cuda.current_device()):
+            raise ValueError(f"gpus[0] must be the network's device {device}, got gpus = {gpus}")
+    poses = torch.as_tensor(poses)
+    if poses.dim() != 3 or tuple(poses.shape[1:]) != (4, 4) or poses.shape[0] < 1:
+        raise ValueError(f"poses must be (V, 4, 4) with V >= 1, got {tuple(poses.shape)}")
+    reso = [int(r) for r in reso]
+    if len(reso) != 3 or min(reso) < 2:
+        raise ValueError(f"reso must be 3 sizes >= 2, got {reso}")
+    lo, hi = np.array(c1, dtype=np.float64), np.array(c2, dtype=np.float64)
+    h = (hi - lo) / (np.array(reso) - 1)
+    if trunc is None:
+        trunc = 3.0 * np.sqrt(3.0) * float(np.abs(h).max())
+    if not 0 < trunc < np.inf:
+        raise ValueError(f"trunc must be positive and finite, got {trunc}")
+    if not 0 < min_opacity <= 1:
+        raise ValueError(f"min_opacity must be in (0, 1], got {min_opacity}")
+    V, W, H = poses.shape[0], int(width), int(height)
+    fx, fy, cx, cy = _intrinsics(W, H, torch.as_tensor(focal).squeeze(), c)
+    bs = max(1, int(ray_batch_size))
+    is_train, renderer_train = net.training, renderer.training
+    net.eval()
+    renderer.eval()
+    try:
+        with torch.no_grad():
+            poses32 = poses.to(device=device, dtype=torch.float32).contiguous()
+            render_par = renderer.bind_parallel(net, gpus)
+            total = V * H * W
+            print("Rendering", V, "views @", total, "rays")
+            depth = torch.empty(V, H, W, dtype=torch.float32, device=device)
+            opacity = torch.empty(V, H, W, dtype=torch.float32, device=device)
+            rays = torch.empty(min(bs, total), 8, dtype=torch.float32, device=device)
+            for first in range(0, total, bs):
+                count = min(bs, total - first)
+                batch = rays[:count]
+                pn.gen_rays(poses32, W, H, fx, fy, cx, cy, z_near, z_far, first, count, out=batch)
+                out = render_par(batch[None], want_weights=True)
+                kept = out["fine"] if renderer.using_fine else out["coarse"]
+                depth.view(-1)[first:first + count] = kept["depth"][0]
+                opacity.view(-1)[first:first + count] = kept["weights"][0].sum(-1)
+            del render_par, rays
+            print("Fusing", V, "views into", reso)
+            tsdf = pn.tsdf_fuse(depth, opacity, poses32, fx, fy, cx, cy, lo, hi, reso, trunc, min_opacity)
+            print("Running marching cubes")
+            vol = -tsdf                                          # inside is positive, as marching cubes takes it
+            if not return_colors:
+                vertices, triangles = pn.marching_cubes(vol, 0.0)
+            else:
+                vertices, triangles, normals, xyz, vd = pn.marching_cubes(vol, 0.0, bounds=(lo, hi))
+                print("Evaluating colour @", len(xyz), "vertices")
+                rgb = _colours(net, xyz, vd, bs, not renderer.using_fine, device)
+                normals, rgb = normals.cpu().numpy(), rgb.cpu().numpy()
+            vertices, triangles = vertices.cpu().numpy(), triangles.cpu().numpy()
+    finally:
+        net.train(is_train)
+        renderer.train(renderer_train)
+    vertices = vertices * h + lo
+    if return_colors:
+        return vertices, triangles, normals, rgb
+    return vertices, triangles
 
 
 def _scaled(vertices, triangles, c1, c2, reso, *colors):

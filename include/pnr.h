@@ -617,6 +617,32 @@ int pnr_tsdf_fuse(const float* depth, const float* opacity, int32_t V, int32_t W
                   float fx, float fy, float cx, float cy, const double* lo, const double* hi, const int32_t* reso,
                   double trunc, double min_opacity, float* tsdf, void* stream);
 
+/* Vertex colours from rendered views (no counterpart in the reference; util/recon.py fuse_views(colors="views")): each
+ * vertex gets the weighted mean of the rendered pixels of the views that see it, under pnr_tsdf_fuse's visibility.
+ * xyz, normals [n][3] float64 (DEVICE: world-space vertices and their unit outward normals); rgb [V][H][W][3], depth
+ * and opacity [V][H][W] fp32 (DEVICE: the renderer's rgb, sum(w z) and weights.sum(-1) of each pixel, the pixel order
+ * of pnr_gen_rays); poses_c2w [V][4][4] fp32 (DEVICE); fx, fy, cx, cy: HOST floats, as pnr_tsdf_fuse.  One thread per
+ * vertex, the views in order, no atomics: repeated calls give the same bits.  All in float64 with round-to-nearest
+ * intrinsics.  Per view v, with R = pose[:3, :3], t = pose[:3, 3], vertex x and normal n:
+ *   q, px, py and the pixel as pnr_tsdf_fuse (the same device code); q_z >= 0 or outside the image: skip v.
+ *   a = opacity of that pixel.  a < min_opacity (or NaN): the pixel saw background, which has no surface colour;
+ *   skip v.
+ *   s = (depth / a - d) / trunc with d = sqrt((q_x^2 + q_y^2) + q_z^2).  |s| > 1 (or NaN): v sees another surface
+ *   (occluded) or this one elsewhere; skip v.
+ *   cos = ((n_0 e_0 + n_1 e_1) + n_2 e_2) / d with e = t - x.  cos <= 0 (or NaN): v faces the back of the surface;
+ *   skip v.
+ *   c_k = (rgb_k - background (1 - a)) / a per channel, then clamped to [0, 1] (NaN -> 0): the renderer composites
+ *   sum(w c) + background (1 - sum(w)), so this is the ray's mean surface colour sum(w c) / sum(w).
+ *   sum_c += cos c, sum_w += cos (in view order).
+ * rgb_out [n][3] fp32 (DEVICE) = sum_c / sum_w rounded to fp32, NaN where no view painted the vertex; weight_out [n]
+ * float64 (DEVICE) = sum_w, 0 where no view painted it.  background: 1 for a white_bkgd renderer, else 0.
+ * Errors (before any CUDA call): NULL pointers, n < 0, V, W or H < 1, trunc not positive and finite, min_opacity
+ * outside (0, 1], background not finite -> PNR_ERR_INVALID.  n = 0 launches nothing. */
+int pnr_paint_vertices(const double* xyz, const double* normals, int64_t n, const float* rgb, const float* depth,
+                       const float* opacity, int32_t V, int32_t W, int32_t H, const float* poses_c2w, float fx,
+                       float fy, float cx, float cy, double trunc, double min_opacity, double background,
+                       float* rgb_out, double* weight_out, void* stream);
+
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.
  * engine = PNR_ENGINE_SIMT: fp32 FFMA SGEMM; PNR_ENGINE_TC (or AUTO): split-bf16 wgmma GEMM (3 products, fp32

@@ -820,6 +820,31 @@ static int band_mc_setup(const int32_t* reso, int32_t block, int32_t apron, cons
 static unsigned grid_for(int64_t n) { return (unsigned)((n + kPtThreads - 1) / kPtThreads); }
 
 // ---- TSDF fusion ---------------------------------------------------------------------------------------------------
+// The pixel of the camera-to-world pose P (row-major 4x4: R = P[:3, :3], t = P[:3, 3]) that the world point x projects
+// to, by the rule of include/pnr.h pnr_tsdf_fuse: d = x - t, q = R^T d, the inverse of pnr_gen_rays, rounded to the
+// nearest pixel with ties up.  -> false when x is behind the camera (or on its plane) or outside the image; else
+// *pix = the pixel's index within the view.  pnr_tsdf_fuse and pnr_paint_vertices share it, so they agree on what
+// every view sees.
+__device__ __forceinline__ bool project_pixel(const float* P, const double x[3], double fx, double fy, double cx,
+                                              double cy, int W, int H, double d[3], double q[3], int64_t* pix) {
+  for (int j = 0; j < 3; ++j) d[j] = __dsub_rn(x[j], (double)P[4 * j + 3]);
+  for (int j = 0; j < 3; ++j)
+    q[j] = __dadd_rn(__dadd_rn(__dmul_rn((double)P[j], d[0]), __dmul_rn((double)P[4 + j], d[1])),
+                     __dmul_rn((double)P[8 + j], d[2]));
+  if (!(q[2] < 0.0)) return false;
+  const double px = __dadd_rn(cx, __ddiv_rn(__dmul_rn(fx, q[0]), -q[2]));
+  const double py = __dadd_rn(cy, __ddiv_rn(__dmul_rn(fy, q[1]), q[2]));
+  const double rx = floor(__dadd_rn(px, 0.5)), ry = floor(__dadd_rn(py, 0.5));    // ties round up
+  if (!(rx >= 0.0 && rx <= (double)(W - 1) && ry >= 0.0 && ry <= (double)(H - 1))) return false;
+  *pix = (int64_t)(int)ry * W + (int)rx;
+  return true;
+}
+
+// |q| as both rules sum it: (q_x^2 + q_y^2) + q_z^2
+__device__ __forceinline__ double ray_distance(const double q[3]) {
+  return sqrt(__dadd_rn(__dadd_rn(__dmul_rn(q[0], q[0]), __dmul_rn(q[1], q[1])), __dmul_rn(q[2], q[2])));
+}
+
 // One thread per voxel (pnr_grid_points' point, in float64), the views in order, the rule of include/pnr.h
 // pnr_tsdf_fuse.  Every operation is one float64 round-to-nearest step, so oracle/pnr_recon_fuse.py gets the same bits.
 __global__ void k_tsdf_fuse(const float* __restrict__ depth, const float* __restrict__ opacity, int V, int W, int H,
@@ -837,24 +862,15 @@ __global__ void k_tsdf_fuse(const float* __restrict__ depth, const float* __rest
   int n = 0;
   bool seen = false;
   for (int v = 0; v < V; ++v) {
-    const float* P = poses + (int64_t)v * 16;          // camera-to-world, row-major 4x4: R = P[:3, :3], t = P[:3, 3]
-    const double d[3] = {__dsub_rn(x[0], (double)P[3]), __dsub_rn(x[1], (double)P[7]), __dsub_rn(x[2], (double)P[11])};
-    double q[3];                                       // R^T (x - t)
-    for (int j = 0; j < 3; ++j)
-      q[j] = __dadd_rn(__dadd_rn(__dmul_rn((double)P[j], d[0]), __dmul_rn((double)P[4 + j], d[1])),
-                       __dmul_rn((double)P[8 + j], d[2]));
-    if (!(q[2] < 0.0)) continue;                       // behind the camera (or on its plane)
-    const double px = __dadd_rn(cx, __ddiv_rn(__dmul_rn(fx, q[0]), -q[2]));
-    const double py = __dadd_rn(cy, __ddiv_rn(__dmul_rn(fy, q[1]), q[2]));
-    const double rx = floor(__dadd_rn(px, 0.5)), ry = floor(__dadd_rn(py, 0.5));    // ties round up
-    if (!(rx >= 0.0 && rx <= (double)(W - 1) && ry >= 0.0 && ry <= (double)(H - 1))) continue;
+    double d[3], q[3];
+    int64_t pix;
+    if (!project_pixel(poses + (int64_t)v * 16, x, fx, fy, cx, cy, W, H, d, q, &pix)) continue;
     seen = true;
-    const int64_t pix = ((int64_t)v * H + (int)ry) * W + (int)rx;
+    pix += (int64_t)v * H * W;
     const double a = (double)opacity[pix];
     double s = 1.0;                                    // background: free space
     if (a >= min_opacity) {
-      const double dist = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(q[0], q[0]), __dmul_rn(q[1], q[1])), __dmul_rn(q[2], q[2])));
-      s = __ddiv_rn(__dsub_rn(__ddiv_rn((double)depth[pix], a), dist), trunc);
+      s = __ddiv_rn(__dsub_rn(__ddiv_rn((double)depth[pix], a), ray_distance(q)), trunc);
       if (!(s >= -1.0)) continue;                      // occluded (or NaN): no observation
       if (s > 1.0) s = 1.0;
     }
@@ -862,6 +878,47 @@ __global__ void k_tsdf_fuse(const float* __restrict__ depth, const float* __rest
     ++n;
   }
   tsdf[p] = n > 0 ? __double2float_rn(__ddiv_rn(sum, (double)n)) : (seen ? -1.0f : 1.0f);
+}
+
+// ---- vertex colours from the rendered views -------------------------------------------------------------------------
+// One thread per vertex, the views in order, the rule of include/pnr.h pnr_paint_vertices.  Every operation is one
+// float64 round-to-nearest step, so oracle/pnr_recon_paint.py gets the same bits.
+__global__ void k_paint_vertices(const double* __restrict__ xyz, const double* __restrict__ normals, int64_t n_verts,
+                                 const float* __restrict__ rgb, const float* __restrict__ depth,
+                                 const float* __restrict__ opacity, int V, int W, int H,
+                                 const float* __restrict__ poses, double fx, double fy, double cx, double cy,
+                                 double trunc, double min_opacity, double background, float* __restrict__ rgb_out,
+                                 double* __restrict__ weight_out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_verts) return;
+  const double x[3] = {xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2]};
+  const double nrm[3] = {normals[3 * i], normals[3 * i + 1], normals[3 * i + 2]};
+  double sum_c[3] = {0.0, 0.0, 0.0}, sum_w = 0.0;
+  for (int v = 0; v < V; ++v) {
+    double d[3], q[3];
+    int64_t pix;
+    if (!project_pixel(poses + (int64_t)v * 16, x, fx, fy, cx, cy, W, H, d, q, &pix)) continue;
+    pix += (int64_t)v * H * W;
+    const double a = (double)opacity[pix];
+    if (!(a >= min_opacity)) continue;                 // background (or NaN): no surface colour
+    const double dist = ray_distance(q);
+    const double s = __ddiv_rn(__dsub_rn(__ddiv_rn((double)depth[pix], a), dist), trunc);
+    if (!(s >= -1.0 && s <= 1.0)) continue;            // occluded, or this view's surface is elsewhere (or NaN)
+    // cos = n . (t - x) / |q|, with t - x = -d exactly
+    const double cosv = __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(nrm[0], -d[0]), __dmul_rn(nrm[1], -d[1])),
+                                            __dmul_rn(nrm[2], -d[2])), dist);
+    if (!(cosv > 0.0)) continue;                       // the back of the surface (or NaN)
+    const double bg = __dmul_rn(background, __dsub_rn(1.0, a));
+    for (int k = 0; k < 3; ++k) {
+      double c = __ddiv_rn(__dsub_rn((double)rgb[3 * pix + k], bg), a);    // un-mix the background
+      if (!(c > 0.0)) c = 0.0;                         // (NaN -> 0)
+      if (c > 1.0) c = 1.0;
+      sum_c[k] = __dadd_rn(sum_c[k], __dmul_rn(cosv, c));
+    }
+    sum_w = __dadd_rn(sum_w, cosv);
+  }
+  for (int k = 0; k < 3; ++k) rgb_out[3 * i + k] = sum_w > 0.0 ? __double2float_rn(__ddiv_rn(sum_c[k], sum_w)) : NAN;
+  weight_out[i] = sum_w;
 }
 
 }  // namespace pnr
@@ -1149,6 +1206,25 @@ int pnr_tsdf_fuse(const float* depth, const float* opacity, int32_t V, int32_t W
   k_tsdf_fuse<<<grid_for(N), kPtThreads, 0, (cudaStream_t)stream>>>(
       depth, opacity, V, W, H, poses_c2w, (double)fx, (double)fy, (double)cx, (double)cy, lo[0], lo[1], lo[2], hi[0],
       hi[1], hi[2], reso[0], reso[1], reso[2], trunc, min_opacity, tsdf);
+  PNR_LAUNCH_CHECK();
+  return PNR_OK;
+}
+
+int pnr_paint_vertices(const double* xyz, const double* normals, int64_t n, const float* rgb, const float* depth,
+                       const float* opacity, int32_t V, int32_t W, int32_t H, const float* poses_c2w, float fx,
+                       float fy, float cx, float cy, double trunc, double min_opacity, double background,
+                       float* rgb_out, double* weight_out, void* stream) {
+  PNR_CHECK_ARG(xyz && normals && rgb && depth && opacity && poses_c2w && rgb_out && weight_out, "NULL pointer");
+  PNR_CHECK_ARG(n >= 0, "negative vertex count");
+  PNR_CHECK_ARG(V >= 1 && W >= 1 && H >= 1, "V, W and H must be >= 1");
+  PNR_CHECK_ARG(trunc > 0.0 && trunc <= 1.7976931348623157e308, "trunc must be positive and finite");
+  PNR_CHECK_ARG(min_opacity > 0.0 && min_opacity <= 1.0, "min_opacity must be in (0, 1]");
+  PNR_CHECK_ARG(background >= -1.7976931348623157e308 && background <= 1.7976931348623157e308,
+                "background must be finite");
+  if (n == 0) return PNR_OK;
+  k_paint_vertices<<<grid_for(n), kPtThreads, 0, (cudaStream_t)stream>>>(
+      xyz, normals, n, rgb, depth, opacity, V, W, H, poses_c2w, (double)fx, (double)fy, (double)cx, (double)cy, trunc,
+      min_opacity, background, rgb_out, weight_out);
   PNR_LAUNCH_CHECK();
   return PNR_OK;
 }

@@ -201,8 +201,10 @@ def declare(L):
                                                vp, sz, vp]
         L.pnr_tsdf_fuse.argtypes = [vp, vp, i32, i32, i32, vp, f32, f32, f32, f32, P(f64), P(f64), P(i32), f64, f64,
                                     vp, vp]
+        L.pnr_paint_vertices.argtypes = [vp, vp, i64, vp, vp, vp, i32, i32, i32, vp, f32, f32, f32, f32, f64, f64, f64,
+                                         vp, vp, vp]
         for name in ("pnr_band_lattice_points", "pnr_band_plan", "pnr_band_points", "pnr_band_mc_count",
-                     "pnr_band_mc_emit", "pnr_band_mc_vertex_attrs", "pnr_tsdf_fuse"):
+                     "pnr_band_mc_emit", "pnr_band_mc_vertex_attrs", "pnr_tsdf_fuse", "pnr_paint_vertices"):
             getattr(L, name).restype = C.c_int
     L.pnr_set_deterministic.argtypes = [C.c_int]
     L.pnr_set_deterministic.restype = C.c_int
@@ -412,6 +414,44 @@ def tsdf_fuse(depth, opacity, poses, fx, fy, cx, cy, lo, hi, reso, trunc, min_op
                                   float(fx), float(fy), float(cx), float(cy), *_bounds3(lo, hi), _reso3(reso),
                                   float(trunc), float(min_opacity), dptr(tsdf), stream_ptr(dev)))
     return tsdf
+
+
+def paint_vertices(xyz, normals, rgb, depth, opacity, poses, fx, fy, cx, cy, trunc, min_opacity, background):
+    """pnr_paint_vertices: world-space vertices and unit outward normals [n, 3] float64, rendered maps rgb [V, H, W, 3],
+    depth and opacity [V, H, W] and camera-to-world poses [V, 4, 4] (fp32), all CUDA tensors on one device -> (rgb
+    [n, 3] fp32, weight [n] float64) on that device: the cos-weighted mean of the pixels of the views that see each
+    vertex, NaN and 0 where none does (rule: include/pnr.h)."""
+    if depth.dim() != 3 or opacity.shape != depth.shape:
+        raise RuntimeError(f"paint_vertices: depth and opacity must both be [V, H, W], got {tuple(depth.shape)} and "
+                           f"{tuple(opacity.shape)}")
+    V, H, W = depth.shape
+    if tuple(rgb.shape) != (V, H, W, 3):
+        raise RuntimeError(f"paint_vertices: rgb must be [{V}, {H}, {W}, 3], got {tuple(rgb.shape)}")
+    if tuple(poses.shape) != (V, 4, 4):
+        raise RuntimeError(f"paint_vertices: poses must be [{V}, 4, 4], got {tuple(poses.shape)}")
+    if xyz.dim() != 2 or xyz.shape[1] != 3 or normals.shape != xyz.shape:
+        raise RuntimeError(f"paint_vertices: xyz and normals must both be [n, 3], got {tuple(xyz.shape)} and "
+                           f"{tuple(normals.shape)}")
+    dev = depth.device
+    for t, name in ((xyz, "xyz"), (normals, "normals"), (rgb, "rgb"), (opacity, "opacity"), (poses, "poses")):
+        if t.device != dev:
+            raise RuntimeError(f"paint_vertices: {name} is on {t.device}, the maps on {dev}")
+    for t, name in ((xyz, "xyz"), (normals, "normals")):
+        if not (t.dtype == torch.float64 and t.is_contiguous()):
+            raise RuntimeError(f"paint_vertices: {name} must be a contiguous float64 tensor, got {t.dtype} "
+                               f"(contiguous={t.is_contiguous()})")
+    n = xyz.shape[0]
+    out = torch.empty(n, 3, dtype=torch.float32, device=dev)
+    weight = torch.empty(n, dtype=torch.float64, device=dev)
+    if n == 0:
+        return out, weight
+    with torch.cuda.device(dev):
+        check(lib().pnr_paint_vertices(C.c_void_p(xyz.data_ptr()), C.c_void_p(normals.data_ptr()), n,
+                                       dptr(rgb, "rgb"), dptr(depth, "depth"), dptr(opacity, "opacity"), V, W, H,
+                                       dptr(poses, "poses"), float(fx), float(fy), float(cx), float(cy), float(trunc),
+                                       float(min_opacity), float(background), dptr(out),
+                                       C.c_void_p(weight.data_ptr()), stream_ptr(dev)))
+    return out, weight
 
 
 BAND_MAX_BLOCK = 256

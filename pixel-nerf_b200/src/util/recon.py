@@ -9,7 +9,8 @@ lattice first and only the blocks the surface crosses are refined and meshed (`p
 pass is sharded over several GPUs (`pnr_mgpu_field_eval`) and the rest stays on the first.  There is no CPU path.
 
 `fuse_views` meshes what the renderer shows instead: it renders depth and opacity maps from camera poses, fuses them
-into a TSDF (`pnr_tsdf_fuse`) and meshes that with the same marching cubes.
+into a TSDF (`pnr_tsdf_fuse`) and meshes that with the same marching cubes.  With `colors="views"` it also paints each
+vertex with the rendered pixels of the views that see it (`pnr_paint_vertices`).
 """
 import warnings
 
@@ -145,6 +146,7 @@ def fuse_views(
     ray_batch_size=50000,
     gpus=None,
     return_colors=False,
+    colors="field",
 ):
     """
     Mesh the surface the renderer shows: render depth and opacity maps of every view, fuse them into a truncated
@@ -161,19 +163,33 @@ def fuse_views(
     :param trunc truncation distance (world units); default 3 voxel diagonals of the coarsest axis
     :param min_opacity a pixel of lower opacity saw background, which carves the voxels it sees
     :param gpus None or a list of CUDA device indices with gpus[0] net's device: the rendering is sharded over them
-    (bind_parallel); fusion, marching cubes and colours run on gpus[0]
+    (bind_parallel); fusion, marching cubes, painting and colours run on gpus[0]
     :param return_colors also return per-vertex normals and colours
+    :param colors where the colours come from (needs return_colors for anything but the default):
+    "field" (default): channels 0-2 of net at the vertex, seen head-on from outside (view direction -normal), from the
+    network of the kept pass, as marching_cubes colours its vertices.
+    "views": the rendered pixels of the views that see the vertex (pnr_paint_vertices, include/pnr.h), from the kept
+    pass's rgb of the same renders, so no extra rendering.  Per view, the vertex's pixel must be a surface pixel
+    (opacity >= min_opacity) whose depth lies within trunc of the vertex (not occluded), and the view must face the
+    surface; the pixel's colour, with the renderer's background un-mixed ((rgb - bkgd (1 - opacity)) / opacity, bkgd = 1
+    for renderer.white_bkgd, else 0), counts with weight cos(normal, direction to the camera).  A vertex no view paints
+    falls back to its "field" colour.  The colours are what the renders show, including any view dependence.
     :return vertices (N, 3) float64 numpy in world coordinates at their true positions, lo + v (hi - lo) / (n - 1)
     for index coordinate v (unlike marching_cubes, which keeps the reference's (c2 - c1) / reso scale); triangles
     (M, 3) int64 numpy, counter-clockwise seen from outside.  With return_colors, also normals (N, 3) float64 numpy,
-    unit, outward (pnr_mc_vertex_attrs on the fused volume), and rgb (N, 3) float32 numpy: channels 0-2 of net at the
-    vertex, seen head-on from outside, from the network of the kept pass.  The fusion rule is pnr_tsdf_fuse's
-    (include/pnr.h): the renderer's depth is sum(w z), so the surface distance of a pixel is depth / opacity.
+    unit, outward (pnr_mc_vertex_attrs on the fused volume), and rgb (N, 3) float32 numpy in [0, 1], from `colors`.
+    The fusion rule is pnr_tsdf_fuse's (include/pnr.h): the renderer's depth is sum(w z), so the surface distance of a
+    pixel is depth / opacity.
 
     Example, a turntable at 30 degrees elevation around an object at the origin::
 
         poses = torch.stack([util.pose_spherical(a, -30.0, 1.3) for a in np.linspace(-180, 180, 65)[:-1]]).cuda()
         verts, tris = util.recon.fuse_views(net, renderer, poses, 128, 128, focal, 0.8, 1.8, reso=[256] * 3)
+
+    and coloured from those renders::
+
+        verts, tris, normals, rgb = util.recon.fuse_views(net, renderer, poses, 128, 128, focal, 0.8, 1.8,
+                                                          reso=[256] * 3, return_colors=True, colors="views")
     """
     from util.util import _intrinsics
     device = next(net.parameters()).device
@@ -199,6 +215,11 @@ def fuse_views(
         raise ValueError(f"trunc must be positive and finite, got {trunc}")
     if not 0 < min_opacity <= 1:
         raise ValueError(f"min_opacity must be in (0, 1], got {min_opacity}")
+    if colors not in ("field", "views"):
+        raise ValueError(f'colors must be "field" or "views", got {colors!r}')
+    if colors == "views" and not return_colors:
+        raise ValueError('colors="views" needs return_colors=True')
+    paint = colors == "views"
     V, W, H = poses.shape[0], int(width), int(height)
     fx, fy, cx, cy = _intrinsics(W, H, torch.as_tensor(focal).squeeze(), c)
     bs = max(1, int(ray_batch_size))
@@ -213,6 +234,7 @@ def fuse_views(
             print("Rendering", V, "views @", total, "rays")
             depth = torch.empty(V, H, W, dtype=torch.float32, device=device)
             opacity = torch.empty(V, H, W, dtype=torch.float32, device=device)
+            rgb_map = torch.empty(V, H, W, 3, dtype=torch.float32, device=device) if paint else None
             rays = torch.empty(min(bs, total), 8, dtype=torch.float32, device=device)
             for first in range(0, total, bs):
                 count = min(bs, total - first)
@@ -222,6 +244,8 @@ def fuse_views(
                 kept = out["fine"] if renderer.using_fine else out["coarse"]
                 depth.view(-1)[first:first + count] = kept["depth"][0]
                 opacity.view(-1)[first:first + count] = kept["weights"][0].sum(-1)
+                if paint:
+                    rgb_map.view(-1, 3)[first:first + count] = kept["rgb"][0]
             del render_par, rays
             print("Fusing", V, "views into", reso)
             tsdf = pn.tsdf_fuse(depth, opacity, poses32, fx, fy, cx, cy, lo, hi, reso, trunc, min_opacity)
@@ -231,14 +255,26 @@ def fuse_views(
                 vertices, triangles = pn.marching_cubes(vol, 0.0)
             else:
                 vertices, triangles, normals, xyz, vd = pn.marching_cubes(vol, 0.0, bounds=(lo, hi))
-                print("Evaluating colour @", len(xyz), "vertices")
-                rgb = _colours(net, xyz, vd, bs, not renderer.using_fine, device)
+            vertices, triangles = vertices.cpu().numpy() * h + lo, triangles.cpu().numpy()
+            if return_colors:
+                coarse = not renderer.using_fine
+                if not paint:
+                    print("Evaluating colour @", len(xyz), "vertices")
+                    rgb = _colours(net, xyz, vd, bs, coarse, device)
+                else:
+                    # the returned world-space vertices; the rows no view paints take the field colour
+                    rgb, weight = pn.paint_vertices(torch.from_numpy(vertices).to(device), normals, rgb_map, depth,
+                                                    opacity, poses32, fx, fy, cx, cy, trunc, min_opacity,
+                                                    1.0 if renderer.white_bkgd else 0.0)
+                    rest = torch.nonzero(weight == 0).view(-1)
+                    print("Painted", len(xyz) - len(rest), "vertices from the views;", len(rest),
+                          "seen by none take the field's colour")
+                    if len(rest):
+                        rgb[rest] = _colours(net, xyz[rest], vd[rest], bs, coarse, device)
                 normals, rgb = normals.cpu().numpy(), rgb.cpu().numpy()
-            vertices, triangles = vertices.cpu().numpy(), triangles.cpu().numpy()
     finally:
         net.train(is_train)
         renderer.train(renderer_train)
-    vertices = vertices * h + lo
     if return_colors:
         return vertices, triangles, normals, rgb
     return vertices, triangles

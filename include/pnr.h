@@ -643,6 +643,42 @@ int pnr_paint_vertices(const double* xyz, const double* normals, int64_t n, cons
                        float fy, float cx, float cy, double trunc, double min_opacity, double background,
                        float* rgb_out, double* weight_out, void* stream);
 
+/* Connected components of a triangle mesh (no counterpart in the reference; util/recon.py keep_components), in two
+ * steps that share one workspace of pnr_mesh_workspace_bytes(n_verts, n_tris) bytes on one stream.  tris [n_tris][3]
+ * int64 vertex ids (DEVICE).  Two vertices are connected when some triangle uses both; a component is a maximal
+ * connected set of vertices with its triangles.  The meshes of pnr_mc_emit are welded, so this is their connectivity.
+ *   pnr_mesh_components  label [n_verts] int64 (DEVICE) = the smallest vertex id of each vertex's component (a vertex
+ *                        no triangle uses is its own component); tri_count [n_verts] int64 (DEVICE) = at a component's
+ *                        label, its number of triangles, 0 at every other index; *counts_out (HOST int64) = the number
+ *                        of components with at least one triangle.  Lock-free union-find over the edges (a, b), (a, c)
+ *                        of each triangle: a root is only ever hooked under a smaller root (64-bit atomicCAS), so every
+ *                        root is its component's minimum whatever the order the threads run in, then one full path
+ *                        compression and integer atomicAdd counts.  The result is one function of the input:
+ *                        repeated calls give the same bits.  Synchronises the stream once, to download the count and
+ *                        the device-side check of the ids.
+ *   pnr_mesh_compact_count  keep_root [n_verts] uint8 (DEVICE), read at the labels: a vertex is kept when
+ *                        keep_root[label[v]] != 0, a triangle when its first vertex is.  counts_out (int64[2], DEVICE) =
+ *                        kept vertices, kept triangles (exclusive scans of the flags, no atomics); leaves in the
+ *                        workspace the flags and new ids pnr_mesh_compact_emit reads.
+ *   pnr_mesh_compact_emit  after pnr_mesh_compact_count with the same tris / label / keep_root / workspace ->
+ *                        vert_ids [n_keep_verts] int64: the kept vertices' old ids, ascending (new id i is old id
+ *                        vert_ids[i]); tris_out [n_keep_tris][3] int64: the kept triangles in their order, through the
+ *                        new ids (n_keep_* = the counted values).
+ * Errors: n_verts or n_tris negative, NULL pointers where a size is non-zero -> PNR_ERR_INVALID; a vertex id outside
+ * [0, n_verts) -> PNR_ERR_INVALID from pnr_mesh_components (found on the device, reported after its synchronise;
+ * label and tri_count are then unspecified).  The compact steps take the tris pnr_mesh_components accepted and the
+ * label it wrote (a triangle with an id out of range is never kept).  A workspace below pnr_mesh_workspace_bytes ->
+ * PNR_ERR_WORKSPACE.  n_tris = 0 or n_verts = 0 launch no union-find. */
+size_t pnr_mesh_workspace_bytes(int64_t n_verts, int64_t n_tris);
+int pnr_mesh_components(const int64_t* tris, int64_t n_tris, int64_t n_verts, int64_t* label, int64_t* tri_count,
+                        int64_t* counts_out, void* workspace, size_t workspace_bytes, void* stream);
+int pnr_mesh_compact_count(const int64_t* tris, int64_t n_tris, int64_t n_verts, const int64_t* label,
+                           const uint8_t* keep_root, int64_t* counts_out, void* workspace, size_t workspace_bytes,
+                           void* stream);
+int pnr_mesh_compact_emit(const int64_t* tris, int64_t n_tris, int64_t n_verts, int64_t* vert_ids, int64_t* tris_out,
+                          int64_t n_keep_verts, int64_t n_keep_tris, void* workspace, size_t workspace_bytes,
+                          void* stream);
+
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.
  * engine = PNR_ENGINE_SIMT: fp32 FFMA SGEMM; PNR_ENGINE_TC (or AUTO): split-bf16 wgmma GEMM (3 products, fp32

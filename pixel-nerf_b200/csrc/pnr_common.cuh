@@ -160,4 +160,10 @@ int tc_render(const PnrScene& sc, const PnrMlp& mlp_coarse, const PnrMlp& mlp_fi
               const float* proj_fine, const PnrRenderCfg& cfg, const float* rays, const PnrNoise& noise, float* zc,
               float* wc, float* zf, const PnrRenderOut& out, int64_t B, void* ws, size_t ws_bytes, cudaStream_t s);
 
+// ---- exclusive scan of the mesh-extraction kernels (pnr_recon.cu), shared with the mesh components (pnr_mesh.cu) -----
+// out[i] = in[0] + ... + in[i - 1] and *total = the sum (int64, device), in three launches on s; n >= 1.  sums:
+// scan_tile_count(n) int64 of scratch.  Reduce-then-scan, no atomics.
+int64_t scan_tile_count(int64_t n);
+int exclusive_scan(const uint8_t* in, int64_t n, int64_t* sums, int64_t* out, int64_t* total, cudaStream_t s);
+
 }  // namespace pnr

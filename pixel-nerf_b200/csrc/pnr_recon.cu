@@ -353,7 +353,9 @@ static size_t mc_carve(int64_t N, void* base, size_t cap, McWs* w) {
   return a.off;
 }
 
-static int exclusive_scan(const uint8_t* in, int64_t n, int64_t* sums, int64_t* out, int64_t* total, cudaStream_t s) {
+int64_t scan_tile_count(int64_t n) { return (n + kScanTile - 1) / kScanTile; }
+
+int exclusive_scan(const uint8_t* in, int64_t n, int64_t* sums, int64_t* out, int64_t* total, cudaStream_t s) {
   const int64_t nb = (n + kScanTile - 1) / kScanTile;
   k_scan_reduce<<<(unsigned)nb, kScanThreads, 0, s>>>(in, n, sums);
   PNR_LAUNCH_CHECK();

@@ -206,6 +206,14 @@ def declare(L):
         for name in ("pnr_band_lattice_points", "pnr_band_plan", "pnr_band_points", "pnr_band_mc_count",
                      "pnr_band_mc_emit", "pnr_band_mc_vertex_attrs", "pnr_tsdf_fuse", "pnr_paint_vertices"):
             getattr(L, name).restype = C.c_int
+    if hasattr(L, "pnr_mesh_components"):  # (not in the host-emulator builds without csrc/pnr_mesh.cu)
+        L.pnr_mesh_workspace_bytes.argtypes = [i64, i64]
+        L.pnr_mesh_workspace_bytes.restype = sz
+        L.pnr_mesh_components.argtypes = [vp, i64, i64, vp, vp, P(i64), vp, sz, vp]
+        L.pnr_mesh_compact_count.argtypes = [vp, i64, i64, vp, vp, vp, vp, sz, vp]
+        L.pnr_mesh_compact_emit.argtypes = [vp, i64, i64, vp, vp, i64, i64, vp, sz, vp]
+        for name in ("pnr_mesh_components", "pnr_mesh_compact_count", "pnr_mesh_compact_emit"):
+            getattr(L, name).restype = C.c_int
     L.pnr_set_deterministic.argtypes = [C.c_int]
     L.pnr_set_deterministic.restype = C.c_int
     L.pnr_get_deterministic.restype = C.c_int
@@ -452,6 +460,66 @@ def paint_vertices(xyz, normals, rgb, depth, opacity, poses, fx, fy, cx, cy, tru
                                        float(min_opacity), float(background), dptr(out),
                                        C.c_void_p(weight.data_ptr()), stream_ptr(dev)))
     return out, weight
+
+
+def _mesh_tris(tris, n_verts):
+    if tris.dim() != 2 or tris.shape[1] != 3 or tris.dtype != torch.int64 or not tris.is_cuda:
+        raise RuntimeError(f"mesh: tris must be an int64 CUDA tensor [M, 3], got {tris.dtype} {tuple(tris.shape)} on "
+                           f"{tris.device}")
+    if int(n_verts) < 0:
+        raise RuntimeError(f"mesh: n_verts must be >= 0, got {n_verts}")
+    return tris.contiguous()
+
+
+def _ptr(t):
+    return C.c_void_p(t.data_ptr()) if t.numel() else None
+
+
+def mesh_components(tris, n_verts):
+    """pnr_mesh_components on an int64 CUDA tensor tris [M, 3] of vertex ids in [0, n_verts) -> (label [n_verts]
+    int64: the smallest vertex id of each vertex's component, tri_count [n_verts] int64: each component's triangles
+    at its label, 0 elsewhere, the number of components with a triangle), on tris' device.  Synchronises once.
+    Raises ValueError for an id outside [0, n_verts) (rule: include/pnr.h)."""
+    tris = _mesh_tris(tris, n_verts)
+    n, m, dev = int(n_verts), tris.shape[0], tris.device
+    L = lib()
+    ws = torch.empty(max(int(L.pnr_mesh_workspace_bytes(n, m)), 1), dtype=torch.uint8, device=dev)
+    label = torch.empty(n, dtype=torch.int64, device=dev)
+    tri_count = torch.empty(n, dtype=torch.int64, device=dev)
+    count = C.c_int64(0)
+    with torch.cuda.device(dev):
+        rc = L.pnr_mesh_components(_ptr(tris), m, n, _ptr(label), _ptr(tri_count), C.byref(count),
+                                   C.c_void_p(ws.data_ptr()), ws.numel(), stream_ptr(dev))
+    if rc == -1 and b"outside [0, n_verts)" in L.pnr_last_error():
+        raise ValueError(f"triangles use a vertex id outside [0, {n})")
+    check(rc)
+    return label, tri_count, count.value
+
+
+def mesh_compact(tris, n_verts, label, keep_root):
+    """pnr_mesh_compact_count + pnr_mesh_compact_emit: the vertices whose root (label) has keep_root [n_verts] uint8
+    set, and the triangles among them -> (vert_ids [K] int64: their old ids ascending, tris [T, 3] int64 through the
+    new ids), on tris' device.  Synchronises once, to size the outputs."""
+    tris = _mesh_tris(tris, n_verts)
+    n, m, dev = int(n_verts), tris.shape[0], tris.device
+    if tuple(label.shape) != (n,) or label.dtype != torch.int64 or label.device != dev:
+        raise RuntimeError(f"mesh_compact: label must be int64 [{n}] on {dev}")
+    if tuple(keep_root.shape) != (n,) or keep_root.dtype != torch.uint8 or keep_root.device != dev:
+        raise RuntimeError(f"mesh_compact: keep_root must be uint8 [{n}] on {dev}")
+    label, keep_root = label.contiguous(), keep_root.contiguous()
+    L = lib()
+    ws = torch.empty(max(int(L.pnr_mesh_workspace_bytes(n, m)), 1), dtype=torch.uint8, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        s = stream_ptr(dev)
+        check(L.pnr_mesh_compact_count(_ptr(tris), m, n, _ptr(label), _ptr(keep_root), C.c_void_p(counts.data_ptr()),
+                                       C.c_void_p(ws.data_ptr()), ws.numel(), s))
+        nv, nt = counts.tolist()
+        vert_ids = torch.empty(nv, dtype=torch.int64, device=dev)
+        tris_out = torch.empty(nt, 3, dtype=torch.int64, device=dev)
+        check(L.pnr_mesh_compact_emit(_ptr(tris), m, n, _ptr(vert_ids), _ptr(tris_out), nv, nt,
+                                      C.c_void_p(ws.data_ptr()), ws.numel(), s))
+    return vert_ids, tris_out
 
 
 BAND_MAX_BLOCK = 256

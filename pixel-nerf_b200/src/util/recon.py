@@ -11,6 +11,9 @@ pass is sharded over several GPUs (`pnr_mgpu_field_eval`) and the rest stays on 
 `fuse_views` meshes what the renderer shows instead: it renders depth and opacity maps from camera poses, fuses them
 into a TSDF (`pnr_tsdf_fuse`) and meshes that with the same marching cubes.  With `colors="views"` it also paints each
 vertex with the rendered pixels of the views that see it (`pnr_paint_vertices`).
+
+`keep_components` drops the floaters either leaves: it labels the mesh's connected components on the GPU
+(`pnr_mesh_components`) and keeps the largest (`pnr_mesh_compact_count` / `pnr_mesh_compact_emit`).
 """
 import warnings
 
@@ -278,6 +281,81 @@ def fuse_views(
     if return_colors:
         return vertices, triangles, normals, rgb
     return vertices, triangles
+
+
+def keep_components(vertices, triangles, *vertex_attrs, largest=1, min_triangles=1, device=None):
+    """
+    Keep the largest connected pieces of a mesh and drop the rest (the floaters of a NeRF field or a fusion), on the
+    GPU.  Composes with both extractors, whatever they return::
+
+        verts, tris, normals, rgb = util.recon.keep_components(
+            *util.recon.fuse_views(net, renderer, poses, ..., return_colors=True, colors="views"), largest=1)
+
+    :param vertices (N, 3) array-like
+    :param triangles (M, 3) array-like of integer vertex ids
+    :param vertex_attrs array-likes with a first dimension of N and any trailing shape and dtype (normals, rgb, ...)
+    :param largest keep at most this many components (>= 1); None keeps every component with min_triangles
+    :param min_triangles keep only components with at least this many triangles (>= 1)
+    :param device the CUDA device to run on (default: the current one); there is no CPU path
+    :return (vertices, triangles, *vertex_attrs) numpy arrays with the input dtypes.
+    Two vertices are connected when some triangle uses both; a component is a maximal connected set of vertices with
+    its triangles (two pieces that touch at one vertex are one component).  A vertex no triangle uses is a component
+    with 0 triangles and is never kept.  Components are ranked by triangle count, descending, ties going to the
+    component whose smallest vertex id is smaller; the first `largest` of that ranking with at least `min_triangles`
+    triangles are kept.  The kept vertices and triangles keep their relative order, the triangles are renumbered to
+    the kept vertices and every attribute is compacted by the same rows; values are copied bit for bit.  So when
+    everything is kept, a mesh without unused vertices (every mesh marching_cubes and fuse_views return) comes back
+    bit-equal.  The labelling is pnr_mesh_components and the compaction pnr_mesh_compact_* (include/pnr.h).
+    Raises ValueError for largest or min_triangles below 1, wrong shapes, an attribute whose first dimension is not N
+    and a triangle id outside [0, N).
+    """
+    for name, v in (("largest", largest), ("min_triangles", min_triangles)):
+        if v is None and name == "largest":
+            continue
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+            raise ValueError(f"{name} must be an int >= 1{' or None' if name == 'largest' else ''}, got {v!r}")
+    vertices, triangles = np.asarray(vertices), np.asarray(triangles)
+    if vertices.ndim != 2 or vertices.shape[1] != 3:
+        raise ValueError(f"vertices must be (N, 3), got {vertices.shape}")
+    if triangles.ndim != 2 or triangles.shape[1] != 3 or not np.issubdtype(triangles.dtype, np.integer):
+        raise ValueError(f"triangles must be (M, 3) integer vertex ids, got {triangles.dtype} {triangles.shape}")
+    N, M = len(vertices), len(triangles)
+    attrs = [np.asarray(a) for a in vertex_attrs]
+    for i, a in enumerate(attrs):
+        if a.ndim < 1 or a.shape[0] != N:
+            raise ValueError(f"vertex_attrs[{i}] must have a first dimension of {N}, got shape {a.shape}")
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if device.type != "cuda":
+        raise RuntimeError(f"keep_components runs on CUDA only (no CPU fallback); got device {device}")
+    with torch.cuda.device(device):
+        tris = torch.from_numpy(np.ascontiguousarray(triangles, dtype=np.int64)).to(device)
+        label, tri_count, n_comp = pn.mesh_components(tris, N)
+        roots = torch.nonzero(tri_count).view(-1)                       # ascending: ties go to the smaller root
+        counts = tri_count[roots]
+        order = torch.sort(counts, descending=True, stable=True).indices
+        ranked, ranked_counts = roots[order], counts[order]
+        kept = ranked[ranked_counts >= int(min_triangles)]
+        if largest is not None:
+            kept = kept[:int(largest)]
+        keep_root = torch.zeros(N, dtype=torch.uint8, device=device)
+        keep_root[kept] = 1
+        vert_ids, tris_out = pn.mesh_compact(tris, N, label, keep_root)
+        del label, tri_count, keep_root, tris
+        out = [_gather(a, vert_ids) for a in [vertices] + attrs]
+        tris_out = tris_out.cpu().numpy().astype(triangles.dtype, copy=False)
+    sep = lambda n: f"{n:,}".replace(",", " ")        # noqa: E731
+    print(f"Kept {len(kept)} of {n_comp} components: {sep(len(tris_out))} of {sep(M)} triangles")
+    return (out[0], tris_out, *out[1:])
+
+
+def _gather(a, rows):
+    """a[rows] for a numpy array a and int64 rows on a CUDA device, gathered there bit for bit, dtype kept."""
+    if len(rows) == 0:
+        return a[:0].copy()
+    if not a.flags.writeable:
+        a = a.copy()
+    t = torch.from_numpy(np.ascontiguousarray(a)).to(rows.device)
+    return t.index_select(0, rows).cpu().numpy()
 
 
 def _scaled(vertices, triangles, c1, c2, reso, *colors):

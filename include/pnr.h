@@ -679,6 +679,52 @@ int pnr_mesh_compact_emit(const int64_t* tris, int64_t n_tris, int64_t n_verts, 
                           int64_t n_keep_verts, int64_t n_keep_tris, void* workspace, size_t workspace_bytes,
                           void* stream);
 
+/* Decimation of a triangle mesh (no counterpart in the reference; util/recon.py decimate, oracle/pnr_recon_decimate.py):
+ * rounds of independent half-edge collapses with Garland-Heckbert quadrics, on one stream, with one workspace of
+ * pnr_decimate_workspace_bytes(n_verts, n_tris) bytes for the initial sizes (it fits every later, smaller round).
+ * xyz [n_verts][3] float64, tris [n_tris][3] int64, quadrics [n_verts][10] float64 (a00 a01 a02 a11 a12 a22 b0 b1 b2 c
+ * of Q(p) = p'Ap + 2b'p + c), all DEVICE.  Every float64 operation rounds to nearest in the order the oracle writes.
+ *   Quadrics  a triangle (p0, p1, p2) has n = (p1 - p0) x (p2 - p0); when |n|^2 > 0 it contributes area * (u u', u d,
+ *             d^2) with u = n / |n|, d = -u.p0, area = |n| / 2, else nothing.  A vertex's quadric is the sum over its
+ *             incident triangles in ascending id (once per corner), starting from 0; a collapse c -> d sets Q_d += Q_c.
+ *             A vertex with more than 64 corners at the start is frozen for the whole call: it is never removed and
+ *             never a d (so its quadric, written as 0, is never read), even after collapses around it take corners
+ *             away.  Cone tips and the poles of UV spheres are such vertices.
+ *   Error     of c -> d: Q = Q_c + Q_d at p_d, err = sqrt(max(Q(p_d), 0) / trace(A)), 0 when trace(A) = 0.
+ *   Vertices  v's corners are its incident triangles, each rotated to (v, x, y); its neighbours are the other ids;
+ *             valence = their number.  A vertex with more than 64 corners in a round is not examined in it:
+ *             valence +inf, no flags.  A frozen vertex has no flags.
+ *             Fan: no incident triangle repeats an id, every neighbour is the x of at most one corner and the y of at
+ *             most one, and the link edges x -> y form one path or one cycle.  Removable: a fan whose link is a cycle
+ *             (closed: every incident edge has two triangles) with 3 to 32 neighbours.
+ *   Valid     c -> d: c removable; d a fan; valence(c) + valence(d) - 4 <= 32; with (c, d, o1) and (c, o2, d) the
+ *             corners of c at d, valence(o1), valence(o2) >= 4 and c, d share no neighbour but o1, o2; no triangle of c
+ *             without d flips (n0 != 0 and n0.n1 <= 0, n1 with c replaced by d); err <= max_error.
+ *   Edge      {a, b} takes its cheaper valid direction, on a tie removing the larger id; key (err, min id, max id).
+ *             best(v) = the smallest key at v, (+inf, INT64_MAX, INT64_MAX) without one.  An edge is selected when it
+ *             is best(a) and best(b) and its key is below best(w) for every other neighbour w of a or b: no two
+ *             selected edges touch or neighbour each other, so a round equals its collapses applied in any order.
+ *   pnr_decimate_init    checks the ids (one synchronise; PNR_ERR_INVALID for an id outside [0, n_verts)) and writes
+ *                        the initial quadrics and frozen [n_verts] uint8 (DEVICE, 1 = frozen), which select reads.
+ *   pnr_decimate_select  -> c_out, d_out [n_verts / 2] int64 and err_out [n_verts / 2] float64 (DEVICE): the selected
+ *                        collapses in ascending c; counts_out (HOST int64[2]) = their number, and 1 when some collapse
+ *                        was valid but for max_error (pass +inf for no bound).  Synchronises once.
+ *   pnr_decimate_apply   the collapses (c[i], d[i]) of one selection (any subset of it): Q_d += Q_c, each c rewritten
+ *                        to its d, each edge cd's two triangles dropped, the rest compacted in order into tris_out
+ *                        [n_tris][3] (not tris); *count_out (HOST) = their number.  Synchronises once.
+ * Errors: negative sizes, NULL pointers where a size is non-zero, a negative or NaN max_error, n_collapses outside
+ * [0, n_verts / 2] -> PNR_ERR_INVALID; a workspace below pnr_decimate_workspace_bytes -> PNR_ERR_WORKSPACE. */
+size_t pnr_decimate_workspace_bytes(int64_t n_verts, int64_t n_tris);
+int pnr_decimate_init(const double* xyz, int64_t n_verts, const int64_t* tris, int64_t n_tris, double* quadrics,
+                      uint8_t* frozen, void* workspace, size_t workspace_bytes, void* stream);
+int pnr_decimate_select(const double* xyz, int64_t n_verts, const int64_t* tris, int64_t n_tris,
+                        const double* quadrics, const uint8_t* frozen, double max_error, int64_t* c_out,
+                        int64_t* d_out, double* err_out, int64_t* counts_out, void* workspace,
+                        size_t workspace_bytes, void* stream);
+int pnr_decimate_apply(const int64_t* tris, int64_t n_tris, int64_t n_verts, const int64_t* c, const int64_t* d,
+                       int64_t n_collapses, double* quadrics, int64_t* tris_out, int64_t* count_out, void* workspace,
+                       size_t workspace_bytes, void* stream);
+
 /* Test hook for the dense contraction the backward path is built from (nn.Linear forward / input gradient / weight
  * gradient are all this "NT" product): C[M][N] (+)= act(A[M][lda]) * W[N][K]^T (+ bias[N]), fp32 in and out.
  * engine = PNR_ENGINE_SIMT: fp32 FFMA SGEMM; PNR_ENGINE_TC (or AUTO): split-bf16 wgmma GEMM (3 products, fp32

@@ -214,6 +214,13 @@ def declare(L):
         L.pnr_mesh_compact_emit.argtypes = [vp, i64, i64, vp, vp, i64, i64, vp, sz, vp]
         for name in ("pnr_mesh_components", "pnr_mesh_compact_count", "pnr_mesh_compact_emit"):
             getattr(L, name).restype = C.c_int
+        L.pnr_decimate_workspace_bytes.argtypes = [i64, i64]
+        L.pnr_decimate_workspace_bytes.restype = sz
+        L.pnr_decimate_init.argtypes = [vp, i64, vp, i64, vp, vp, vp, sz, vp]
+        L.pnr_decimate_select.argtypes = [vp, i64, vp, i64, vp, vp, C.c_double, vp, vp, vp, P(i64), vp, sz, vp]
+        L.pnr_decimate_apply.argtypes = [vp, i64, i64, vp, vp, i64, vp, vp, P(i64), vp, sz, vp]
+        for name in ("pnr_decimate_init", "pnr_decimate_select", "pnr_decimate_apply"):
+            getattr(L, name).restype = C.c_int
     L.pnr_set_deterministic.argtypes = [C.c_int]
     L.pnr_set_deterministic.restype = C.c_int
     L.pnr_get_deterministic.restype = C.c_int
@@ -520,6 +527,59 @@ def mesh_compact(tris, n_verts, label, keep_root):
         check(L.pnr_mesh_compact_emit(_ptr(tris), m, n, _ptr(vert_ids), _ptr(tris_out), nv, nt,
                                       C.c_void_p(ws.data_ptr()), ws.numel(), s))
     return vert_ids, tris_out
+
+
+class Decimator:
+    """The state of one pnr_decimate_* run on a mesh's device: xyz [N, 3] float64, tris [M, 3] int64 (ids checked in
+    [0, N) on the device: ValueError otherwise), the quadrics [N, 10] float64 and a workspace sized for (N, M).
+    select() -> (c, d, err) of one round's selected collapses, ascending c, and whether max_error held some back;
+    apply(c, d) collapses them and returns the new triangle count (rule: include/pnr.h).  Each call synchronises once.
+    The rounds ping-pong between tris and a second buffer, so tris is overwritten: pass a tensor the caller owns."""
+
+    def __init__(self, xyz, tris):
+        tris = _mesh_tris(tris, xyz.shape[0])
+        if xyz.dim() != 2 or xyz.shape[1] != 3 or xyz.dtype != torch.float64 or xyz.device != tris.device:
+            raise RuntimeError(f"decimate: xyz must be float64 [N, 3] on {tris.device}")
+        self.xyz, self.tris, self.dev = xyz.contiguous(), tris, tris.device
+        self.n = n = xyz.shape[0]
+        L = self.L = lib()
+        self.ws = torch.empty(max(int(L.pnr_decimate_workspace_bytes(n, tris.shape[0])), 1), dtype=torch.uint8,
+                              device=self.dev)
+        self.quadrics = torch.empty(n, 10, dtype=torch.float64, device=self.dev)
+        self.frozen = torch.empty(n, dtype=torch.uint8, device=self.dev)
+        self.spare = torch.empty_like(tris)
+        with torch.cuda.device(self.dev):
+            rc = L.pnr_decimate_init(_ptr(self.xyz), n, _ptr(tris), tris.shape[0], _ptr(self.quadrics),
+                                     _ptr(self.frozen), C.c_void_p(self.ws.data_ptr()), self.ws.numel(),
+                                     stream_ptr(self.dev))
+        if rc == -1 and b"outside [0, n_verts)" in L.pnr_last_error():
+            raise ValueError(f"triangles use a vertex id outside [0, {n})")
+        check(rc)
+
+    def select(self, max_error=None):
+        bound = float("inf") if max_error is None else float(max_error)
+        k = max(self.n // 2, 1)                  # (never 0, so that no output is NULL for a 1-vertex mesh)
+        c, d = (torch.empty(k, dtype=torch.int64, device=self.dev) for _ in range(2))
+        err = torch.empty(k, dtype=torch.float64, device=self.dev)
+        counts = (C.c_int64 * 2)()
+        with torch.cuda.device(self.dev):
+            check(self.L.pnr_decimate_select(_ptr(self.xyz), self.n, _ptr(self.tris), self.tris.shape[0],
+                                             _ptr(self.quadrics), _ptr(self.frozen), bound, _ptr(c), _ptr(d), _ptr(err),
+                                             C.cast(counts, C.POINTER(C.c_int64)), C.c_void_p(self.ws.data_ptr()),
+                                             self.ws.numel(), stream_ptr(self.dev)))
+        k = counts[0]
+        return c[:k], d[:k], err[:k], bool(counts[1])
+
+    def apply(self, c, d):
+        c, d = c.contiguous(), d.contiguous()
+        m = self.tris.shape[0]
+        count = C.c_int64(0)
+        with torch.cuda.device(self.dev):
+            check(self.L.pnr_decimate_apply(_ptr(self.tris), m, self.n, _ptr(c), _ptr(d), c.numel(),
+                                            _ptr(self.quadrics), _ptr(self.spare), C.byref(count),
+                                            C.c_void_p(self.ws.data_ptr()), self.ws.numel(), stream_ptr(self.dev)))
+        self.tris, self.spare = self.spare[:count.value], self.tris
+        return count.value
 
 
 BAND_MAX_BLOCK = 256

@@ -14,6 +14,7 @@ vertex with the rendered pixels of the views that see it (`pnr_paint_vertices`).
 
 `keep_components` drops the floaters either leaves: it labels the mesh's connected components on the GPU
 (`pnr_mesh_components`) and keeps the largest (`pnr_mesh_compact_count` / `pnr_mesh_compact_emit`).
+`decimate` then reduces the mesh with rounds of independent quadric edge collapses on the GPU (`pnr_decimate_*`).
 """
 import warnings
 
@@ -345,6 +346,91 @@ def keep_components(vertices, triangles, *vertex_attrs, largest=1, min_triangles
         tris_out = tris_out.cpu().numpy().astype(triangles.dtype, copy=False)
     sep = lambda n: f"{n:,}".replace(",", " ")        # noqa: E731
     print(f"Kept {len(kept)} of {n_comp} components: {sep(len(tris_out))} of {sep(M)} triangles")
+    return (out[0], tris_out, *out[1:])
+
+
+def decimate(vertices, triangles, *vertex_attrs, target_triangles=None, max_error=None, device=None):
+    """
+    Reduce a mesh on the GPU with quadric edge collapses, keeping a subset of its vertices.  Composes with the
+    extractors and keep_components, whatever they return::
+
+        verts, tris, normals, rgb = util.recon.decimate(
+            *util.recon.keep_components(*util.recon.fuse_views(..., return_colors=True, colors="views"), largest=1),
+            target_triangles=200_000)
+
+    :param vertices (N, 3) array-like
+    :param triangles (M, 3) array-like of integer vertex ids
+    :param vertex_attrs array-likes with a first dimension of N and any trailing shape and dtype (normals, rgb, ...)
+    :param target_triangles stop once the mesh has at most this many triangles (>= 0)
+    :param max_error make no collapse whose error exceeds this world length (finite, >= 0); at least one of the two
+        bounds is needed, and with both the call stops at whichever binds first
+    :param device the CUDA device to run on (default: the current one); there is no CPU path
+    :return (vertices, triangles, *vertex_attrs) numpy arrays with the input dtypes.
+    Each collapse removes one vertex c and rewrites its triangles to a neighbour d, which does not move; its error is
+    the area-weighted RMS distance of d from the planes of the triangles merged into it (Garland-Heckbert quadrics).
+    Only interior manifold vertices are removed, so boundaries and non-manifold parts come through unchanged, and no
+    collapse flips a triangle.  A vertex with more than 64 incident triangles (a cone tip, a pole) is always kept.  Each round applies a set of collapses far enough apart not to interact, chosen by
+    smallest error (pnr_decimate_select); a round that would overshoot the target keeps its cheapest collapses, so
+    the result has target - 1 or target triangles unless no valid collapse is left.  The output vertices are input
+    rows in their input order, with every attribute copied bit for bit; the triangles keep their relative order,
+    renumbered to the vertices they use, and unused vertices are dropped.  The rule is in include/pnr.h.
+    Raises ValueError without a bound, for a negative target_triangles, a negative or non-finite max_error, wrong
+    shapes, an attribute whose first dimension is not N and a triangle id outside [0, N).
+    """
+    if target_triangles is None and max_error is None:
+        raise ValueError("decimate needs target_triangles or max_error")
+    if target_triangles is not None and (isinstance(target_triangles, bool) or
+                                         not isinstance(target_triangles, (int, np.integer)) or target_triangles < 0):
+        raise ValueError(f"target_triangles must be an int >= 0, got {target_triangles!r}")
+    if max_error is not None:
+        if isinstance(max_error, bool) or not isinstance(max_error, (int, float, np.integer, np.floating)) or \
+                not np.isfinite(max_error) or max_error < 0:
+            raise ValueError(f"max_error must be a finite number >= 0, got {max_error!r}")
+    vertices, triangles = np.asarray(vertices), np.asarray(triangles)
+    if vertices.ndim != 2 or vertices.shape[1] != 3 or not (np.issubdtype(vertices.dtype, np.floating) or
+                                                             np.issubdtype(vertices.dtype, np.integer)):
+        raise ValueError(f"vertices must be (N, 3) real numbers, got {vertices.dtype} {vertices.shape}")
+    if triangles.ndim != 2 or triangles.shape[1] != 3 or not np.issubdtype(triangles.dtype, np.integer):
+        raise ValueError(f"triangles must be (M, 3) integer vertex ids, got {triangles.dtype} {triangles.shape}")
+    N, M = len(vertices), len(triangles)
+    attrs = [np.asarray(a) for a in vertex_attrs]
+    for i, a in enumerate(attrs):
+        if a.ndim < 1 or a.shape[0] != N:
+            raise ValueError(f"vertex_attrs[{i}] must have a first dimension of {N}, got shape {a.shape}")
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if device.type != "cuda":
+        raise RuntimeError(f"decimate runs on CUDA only (no CPU fallback); got device {device}")
+    with torch.cuda.device(device):
+        xyz = torch.from_numpy(np.ascontiguousarray(vertices, dtype=np.float64)).to(device)
+        tris = torch.from_numpy(np.ascontiguousarray(triangles, dtype=np.int64)).to(device)
+        dec = pn.Decimator(xyz, tris)
+        rounds, m = 0, M
+        while True:
+            if target_triangles is not None and m <= target_triangles:
+                reason = "target reached"
+                break
+            c, d, err, held_back = dec.select(max_error)
+            if len(c) == 0:
+                reason = "error bound" if held_back else "no valid collapse left"
+                break
+            if target_triangles is not None and len(c) > -(-(m - target_triangles) // 2):
+                keep = -(-(m - target_triangles) // 2)
+                # the smallest keys (err, min id, max id); the selected edges share no vertex, so min id decides ties
+                order = torch.sort(torch.minimum(c, d), stable=True).indices
+                order = order[torch.sort(err[order], stable=True).indices[:keep]]
+                order = torch.sort(order).values
+                c, d = c[order], d[order]
+            m = dec.apply(c, d)
+            rounds += 1
+        tris = dec.tris
+        used = torch.zeros(N, dtype=torch.uint8, device=device)
+        used[tris.reshape(-1)] = 1
+        del dec, xyz
+        vert_ids, tris_out = pn.mesh_compact(tris, N, torch.arange(N, device=device), used)
+        out = [_gather(a, vert_ids) for a in [vertices] + attrs]
+        tris_out = tris_out.cpu().numpy().astype(triangles.dtype, copy=False)
+    sep = lambda n: f"{n:,}".replace(",", " ")        # noqa: E731
+    print(f"Decimated in {rounds} rounds: {sep(M)} to {sep(len(tris_out))} triangles ({reason})")
     return (out[0], tris_out, *out[1:])
 
 
